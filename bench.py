@@ -1,15 +1,16 @@
 #!/usr/bin/env python
-"""bench.py — the driver-facing benchmark of the B200 state-root engine.
+"""bench.py — the benchmark of the state-root engine (H100, sm_90a).
 
     python bench.py --gpus N --steps K --warmup W            (N>1: launched under torchrun, one rank per GPU)
     python bench.py --impl reference --gpus N --steps K --warmup W
+    python bench.py --gpus 1 --steps K --warmup W --dump-outputs DIR   (writes what the timed legs returned, see sample_digests)
 
 Headline workload (BASELINE.json configs[1], "C2"): batch keccak256 of 10M 32-byte keys per GPU — the
 AccountHashing / StorageHashing inner loop.  One step = one pass over the batch.
   value : digests/s, inputs resident in HBM, CUDA events on the launching stream, max over ranks
   e2e   : same metric through the C-ABI with HOST (page-locked) buffers, H2D + hash + D2H inside the region
 Objects in the same JSON line (each with its own `roofline`: HBM fraction from the algorithmic bytes of SURVEY.md §8d,
-`alu_frac` against the measured ALU-pipe ceiling, `traffic` from the committed ncu sums in profiles/roofline_traffic.json):
+`alu_frac` against the ALU-pipe ceiling of the device's SMs at the sampled SM clock):
   state_root    C3 (configs[2]): StateRoot over 1M accounts x 16 slots per GPU, leaves/s; at N>1 the accounts are sharded by
                 top key nibble and the 16-entry frontier is all-gathered inside b200_state_root_sharded_dev (NCCL behind the
                 C ABI) — the only collective of the path; e2e through b200_state_root_full with host buffers
@@ -18,8 +19,9 @@ Objects in the same JSON line (each with its own `roofline`: HBM fraction from t
   incremental   C5 (configs[4]): 10k dirty accounts against a resident 100M-leaf trie, latency; the incremental root is
                 checked against a from-scratch device build of the updated state inside the run
   dynamic       the in-place block-update path (b200_dtrie_apply at 100M leaves, mixed blocks; b200_dstate_apply on the C3
-                state) and the f2/f3/f4 legs (hash+sort, ordered roots, table rows), each in its own process and each
-                checking itself (per-block roots against the static path / a twin, and an undo block back to the seed root)
+                state) and the f2/f3/f4 legs (hash+sort, ordered roots, table rows), each in its own process, each timing
+                --steps blocks / repetitions and each checking itself (per-block roots against the static path / a twin,
+                and an undo block back to the seed root)
   cpu_baseline  the oracle's keccak on the host cores, bounded sample; clocks; gpu_launches; parity_spot_check.
 
 --impl reference times the CPU restatement of reth's algorithm (oracle/, all host threads) on the SAME 10M keys and config:
@@ -90,7 +92,7 @@ def c2_config(n_keys: int, world: int) -> dict:
     """`config` of the headline line: the same dict on both arms (the driver compares them)."""
     return {"workload": "C2: batch keccak256 of 10M 32-byte keys per GPU (AccountHashing/StorageHashing inner loop)",
             "keys_per_gpu": n_keys, "msg_len": 32, "parallelism": f"keys sharded over {world} GPU(s), no collective",
-            "l2": "input 320 MB + output 320 MB per step exceed the 126 MB L2; no flush needed"}
+            "l2": "input 320 MB + output 320 MB per step exceed the 50 MB L2; no flush needed"}
 
 
 # ------------------------------------------------------------------------------------------------ synthetic data
@@ -212,37 +214,35 @@ class ClockSampler:
 
 
 # ------------------------------------------------------------------------------------------------ roofline
-ALU_INSTR_PER_KECCAK_F = 4220.0  # ALU-pipe instructions per digest of keccak256_fixed32_kernel counted from its SASS
-                                 # (tools/sass_count.py -> profiles/r02_keccak_sass_count.txt: 132 + 22 x 183 + 62; ncu
-                                 # counts 4286 instructions of all kinds per digest, profiles/r02_keccak32.md)
-ALU_LANES_PER_CLK_PER_SM = 64.0  # measured: profiles/r01_pipe_microbench.txt
+ALU_INSTR_PER_KECCAK_F = 4483.0  # ALU-pipe instructions per digest of keccak256_fixed32_kernel in its sm_90a SASS
+                                 # (tools/sass_count.py: 131 + 22 x 195 + 62)
+ALU_LANES_PER_CLK_PER_SM = 64.0  # 32-bit logic / shift / add lanes per clock per SM on compute capability 9.0
+                                 # (CUDA C++ Programming Guide, arithmetic instruction throughput)
 
 
 def hbm_peak():
     peaks_path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(peaks_path):
         return json.load(open(peaks_path))["hbm_gbs"], "of measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "of fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "of data sheet (H100 SXM HBM3, 3.35 TB/s)"
 
 
-def traffic_of(key):
-    prof = os.path.join(ROOT, "profiles", "roofline_traffic.json")
-    if os.path.exists(prof):
-        return json.load(open(prof)).get(key)
-    return None
+def n_sms() -> int:
+    import torch
+    return torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
 
 
-def make_roofline(algo_bytes: float, seconds: float, keccak_f: float, sm_mhz, traffic_key: str, kernel: str, n_sms: int = 148):
-    """roofline object of one leg: `achieved` = algorithmic bytes (SURVEY.md §8d) / device time against the HBM peak (the
-    contract figure), `alu_frac` = Keccak-f executed / device time against the measured ALU-pipe ceiling (the binding one)."""
+def make_roofline(algo_bytes: float, seconds: float, keccak_f: float, sm_mhz, kernel: str):
+    """roofline object of one leg: `achieved` = algorithmic bytes (SURVEY.md §8d) / device time against the HBM peak,
+    `alu_frac` = Keccak-f executed / device time against the ALU-pipe ceiling at the sampled SM clock (the binding one)."""
     peak, src = hbm_peak()
     achieved = algo_bytes / seconds / 1e9
     r = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-         "traffic": traffic_of(traffic_key), "kernel": kernel, "peak_source": src,
+         "kernel": kernel, "peak_source": src,
          "algorithmic_bytes_per_launch": algo_bytes, "keccak_f_per_launch": keccak_f, "alu_frac": None,
-         "note": "Keccak-f is ALU-bound (~4220 ALU-pipe instructions per permutation on the 64-lane/clk/SM ALU pipe): alu_frac is the binding roofline"}
+         "note": "Keccak-f is ALU-bound (~4483 ALU-pipe instructions per permutation on the 64-lane/clk/SM ALU pipe): alu_frac is the binding roofline"}
     if sm_mhz:
-        alu_peak = n_sms * ALU_LANES_PER_CLK_PER_SM * sm_mhz * 1e6 / ALU_INSTR_PER_KECCAK_F
+        alu_peak = n_sms() * ALU_LANES_PER_CLK_PER_SM * sm_mhz * 1e6 / ALU_INSTR_PER_KECCAK_F
         r["alu_peak_keccak_f_per_s"] = alu_peak
         r["alu_frac"] = (keccak_f / seconds) / alu_peak
     return r
@@ -361,6 +361,8 @@ def main():
     ap.add_argument("--skip-c4", action="store_true")
     ap.add_argument("--c4-leaves", type=int, default=31_250_000, help="leaves per GPU (250M over 8 GPUs)")
     ap.add_argument("--skip-cpu", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write what the timed legs computed in their "
+                    "last step to DIR/<name>.npy (float32 / float64, see sample_digests)")
     ap.add_argument("--skip-dynamic", action="store_true", help="skip the in-place block-update legs (dynamic resident trie / "
                     "state: tools/dtrie_bench.py, tools/dstate_bench.py, each in its own process) and the f2/f3/f4 throughput legs")
     args = ap.parse_args()
@@ -377,8 +379,8 @@ def main():
 
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
-    # one process per GPU: this rank's CPUs and its page-locked staging buffers on the GPU's own socket (SCALE_r01: GPUs 0-3
-    # hang off NUMA node 0, 4-7 off node 1; the e2e leg moves 640 MB per step and GPU through host memory)
+    # one process per GPU: this rank's CPUs and its page-locked staging buffers on the GPU's own NUMA node (the e2e leg moves
+    # 640 MB per step and GPU through host memory)
     from reth_b200 import numa_bind_thread
     numa_node = numa_bind_thread(local_rank)
     if world > 1:
@@ -440,6 +442,7 @@ def main():
     gpu_launches = eng.launch_count() - launches0
     ms_per_step = ms_total / args.steps
     value = world * n * args.steps / (ms_total * 1e-3)
+    dumps = sample_digests(d_out, n) if args.dump_outputs and rank == 0 else None
 
     # spot-check the timed output against the oracle (checker only)
     import oracle
@@ -456,7 +459,7 @@ def main():
     for _ in range(2):
         eng.keccak256_fixed(h_in, 32, out=h_out)
     barrier()
-    e2e_steps = max(3, min(args.steps, 10))
+    e2e_steps = args.steps
     t0 = time.perf_counter()
     for _ in range(e2e_steps):
         eng.keccak256_fixed(h_in, 32, out=h_out)
@@ -469,8 +472,7 @@ def main():
 
     # ---------------------------------------------------------------- roofline of the dominant kernel
     # 32 B key read + 32 B digest written per digest (SURVEY.md §8d); one Keccak-f per digest
-    roofline = make_roofline(64.0 * n, ms_per_step * 1e-3, float(n), clk.summary()["sm_mhz"],
-                             "keccak256_fixed32_kernel_dram_bytes_per_launch", "keccak256_fixed32_kernel")
+    roofline = make_roofline(64.0 * n, ms_per_step * 1e-3, float(n), clk.summary()["sm_mhz"], "keccak256_fixed32_kernel")
     sm_mhz = clk.summary()["sm_mhz"]
 
     # ---------------------------------------------------------------- C3: state root
@@ -498,6 +500,10 @@ def main():
 
     dynamic = None
     if not args.skip_dynamic and rank == 0 and world == 1:
+        # the dynamic legs run in processes of their own and need most of the GPU's 80 GB: release what this one holds
+        del d_keys, d_out
+        eng.close()
+        torch.cuda.empty_cache()
         dynamic = bench_dynamic(args)
 
     if rank == 0:
@@ -513,11 +519,32 @@ def main():
         }
         if dynamic is not None:
             line["dynamic"] = dynamic
+        if dumps is not None:
+            for name, leg in (("state_root", state_root), ("mainnet_shape_root", c4)):
+                if leg is not None:
+                    dumps[name] = np.frombuffer(bytes.fromhex(leg["root"]), np.uint8).astype(np.float32)
+            if incremental is not None and "root_after" in incremental:
+                dumps["incremental_root"] = np.frombuffer(bytes.fromhex(incremental["root_after"]), np.uint8).astype(np.float32)
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            for name, a in dumps.items():
+                np.save(os.path.join(args.dump_outputs, f"{name}.npy"), a)
         emit(line)
     if comm is not None:
         comm.close()
     if world > 1:
         dist.destroy_process_group()
+
+
+DUMP_ROWS = 262_144  # digests kept by --dump-outputs: 262144 x 32 bytes as float32 = 32 MB
+
+
+def sample_digests(d_out, n: int) -> dict:
+    """--dump-outputs of the C2 leg: the digests of its last timed step (bytes as float32) at a fixed, seeded sample of rows
+    (all rows when the batch has at most DUMP_ROWS), and the row numbers (float64).  The state-root legs add their roots."""
+    import torch
+    rows = np.arange(n) if n <= DUMP_ROWS else np.sort(np.random.default_rng(0).choice(n, DUMP_ROWS, replace=False))
+    dig = d_out.view(n, 32)[torch.from_numpy(rows).to(d_out.device)].cpu().numpy()
+    return {"keccak_rows": rows.astype(np.float64), "keccak_digests": dig.astype(np.float32)}
 
 
 def bench_state_root(args, eng, dev, rank, world, barrier, max_over_ranks, sm_mhz=None, comm=None):
@@ -545,7 +572,7 @@ def bench_state_root(args, eng, dev, rank, world, barrier, max_over_ranks, sm_mh
         step()
     barrier()
     eng.dev_status()
-    steps = max(3, min(args.steps, 10))
+    steps = args.steps
     l0 = eng.launch_count()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
@@ -571,7 +598,7 @@ def bench_state_root(args, eng, dev, rank, world, barrier, max_over_ranks, sm_mh
     # the device (stats.keccak_f)
     kf = float(stats.get("keccak_f") or 0) or 1.494 * leaves
     res["roofline"] = make_roofline(float(n_acc * C3_SLOTS * 64 + n_acc * 104), ms * 1e-3, kf, sm_mhz,
-                                    "state_root_c3_dram_bytes_per_step", "state_root_full (leaf + branch kernels of one build)")
+                                    "state_root_full (leaf + branch kernels of one build)")
     if world == 1:
         # e2e: host (page-locked) buffers through b200_state_root_full
         h = {k: eng.pinned_empty(tuple(v.shape), np.uint8 if v.dtype == torch.uint8 else np.int64)
@@ -583,7 +610,7 @@ def bench_state_root(args, eng, dev, rank, world, barrier, max_over_ranks, sm_mh
         for _ in range(2):
             root = eng.state_root_full(h["akeys"], accts, h["skeys"], h["svals"], h["offs"].view(np.uint64))
         t0 = time.perf_counter()
-        e2e_steps = 3
+        e2e_steps = args.steps
         for _ in range(e2e_steps):
             root = eng.state_root_full(h["akeys"], accts, h["skeys"], h["svals"], h["offs"].view(np.uint64))
         dt = time.perf_counter() - t0
@@ -609,7 +636,7 @@ def bench_hash_partition(args, eng, comm, dev, rank, world, barrier, max_over_ra
     for _ in range(2):
         got = comm.hash_partition_dev(t_in, 20, 20, n, t_val, 72, cap, t_k, t_v)
     barrier()
-    steps = 5
+    steps = args.steps
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for _ in range(steps):
@@ -694,7 +721,7 @@ def bench_c4(args, eng, dev, rank, world, barrier, max_over_ranks, comm=None):
         step()
     barrier()
     eng.dev_status()
-    steps = 5
+    steps = args.steps
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for _ in range(steps):
@@ -749,7 +776,7 @@ def bench_incremental(args, eng, dev, sm_mhz=None, skip_cpu=False):
     lat = []
     d_new_root = torch.zeros(32, dtype=torch.uint8, device=dev)
     accts_now = accts  # updated in place as the updates are committed (the base tensor is not needed afterwards)
-    reps = 12
+    reps = 2 + args.steps  # the first two updates are not timed
     for it in range(reps):
         idx = torch.randperm(n, generator=g, device=dev)[:m] if n < 50_000_000 else \
             torch.unique(torch.randint(0, n, (m + m // 8,), generator=g, device=dev))[:m]
@@ -779,9 +806,9 @@ def bench_incremental(args, eng, dev, sm_mhz=None, skip_cpu=False):
     eng.set_stream(None)
     trie.update(hk, ha)
     t0 = time.perf_counter()
-    for _ in range(5):
+    for _ in range(args.steps):
         root = trie.update(hk, ha)
-    e2e_us = (time.perf_counter() - t0) / 5 * 1e6
+    e2e_us = (time.perf_counter() - t0) / args.steps * 1e6
     eng.use_torch_stream()
     # in-bench parity: the incremental root must equal a from-scratch device build of the updated state (the from-scratch
     # path is the one the tests pin against the oracle and reth's golden roots); `accts_now` tracks what was committed
@@ -804,7 +831,7 @@ def bench_incremental(args, eng, dev, sm_mhz=None, skip_cpu=False):
            "root_check": "incremental root == from-scratch device build of the updated 100M-leaf state: ok",
            "rehashed_branch_nodes": stats["branches_added"], "levels": stats["levels"],
            "resident_bytes": trie.device_bytes(),
-           "roofline": make_roofline(algo, dev_us * 1e-6, kf, sm_mhz, "incremental_c5_dram_bytes_per_step",
+           "roofline": make_roofline(algo, dev_us * 1e-6, kf, sm_mhz,
                                      "b200_trie_update (locate + mark + wavefront)"),
            "config": {"workload": f"C5: {mm}-account dirty set against a resident {n}-leaf base trie, "
                                   "value changes of existing accounts, root path re-hash only"}}
@@ -841,15 +868,18 @@ def bench_dynamic(args):
     import subprocess
     root = os.path.dirname(os.path.abspath(__file__))
     out = {}
+    blocks = str(args.steps + 2)   # the block legs time every block but the first two
+    reps = str(args.steps)
     runs = {
         "dtrie_apply_mixed_block": ["tools/dtrie_bench.py", "--base", str(args.base_accounts), "--dirty", str(args.dirty),
-                                    "--mix", "80,10,10", "--compare", "--cpu-sample", "1000000"],
+                                    "--mix", "80,10,10", "--compare", "--cpu-sample", "1000000", "--blocks", blocks],
         "dstate_apply_c3_shape": ["tools/dstate_bench.py", "--accounts", "1000000", "--slots", "16", "--touch", "2000",
-                                  "--slot-writes", "10", "--device-resident", "--cpu-sample", "40000"],
-        "hash_sort_keys": ["tools/hash_sort_bench.py", "--keys", "10000000"],
-        "hash_sort_storage": ["tools/hash_sort_storage_bench.py", "--slots", "10000000", "--accounts", "200000"],
-        "ordered_roots_receipts": ["tools/ordered_bench.py", "--blocks", "2000", "--items", "200", "--shape", "receipts"],
-        "table_rows_c3_shape": ["tools/rows_bench.py", "--accounts", "1000000", "--slots", "16"],
+                                  "--slot-writes", "10", "--device-resident", "--cpu-sample", "40000", "--blocks", blocks],
+        "hash_sort_keys": ["tools/hash_sort_bench.py", "--keys", "10000000", "--reps", reps],
+        "hash_sort_storage": ["tools/hash_sort_storage_bench.py", "--slots", "10000000", "--accounts", "200000", "--reps", reps],
+        "ordered_roots_receipts": ["tools/ordered_bench.py", "--blocks", "2000", "--items", "200", "--shape", "receipts",
+                                   "--reps", reps],
+        "table_rows_c3_shape": ["tools/rows_bench.py", "--accounts", "1000000", "--slots", "16", "--reps", reps],
     }
     for name, cmd in runs.items():
         if not os.path.exists(os.path.join(root, cmd[0])):

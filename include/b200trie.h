@@ -1,5 +1,5 @@
 /*
- * b200trie.h — C ABI of the B200-native state-root engine (libb200trie.so).
+ * b200trie.h — C ABI of the GPU state-root engine (libb200trie.so, built for the H100, sm_90a).
  *
  * This is the drop-in boundary for reth's Merkle-Patricia-Trie commitment path.  reth has no FFI for this
  * path (it is all Rust traits/closures); each entry point below names the reference interface a thin Rust
@@ -461,8 +461,7 @@ B200_API void b200_trie_destroy(b200_trie *);
  * reth's sparse trie on the live path (ParallelSparseTrie::update_leaf / remove_leaf / root,
  * crates/trie/sparse/src/parallel.rs) and of TrieWalker + prefix sets on the database path
  * (crates/trie/trie/src/walker.rs:161-202, crates/trie/common/src/prefix_set.rs).
- * STATUS: validated bit-exact against the oracle under tools/emu (CPU emulation of these kernels); first B200 run
- * pending — until then b200_trie_apply (merge + rebuild) is the measured path.
+ * STATUS: validated bit-exact against the oracle on the GPU (tests/test_gpu_dtrie.py) and under tools/emu.
  *
  * b200_dtrie_apply: keys32 strictly ascending; present[i] == 0 deletes key i (NULL: all upserts); deleting an absent
  * key is a no-op.  storage_roots32 may be NULL (new accounts get EMPTY_ROOT_HASH, existing ones keep theirs).
@@ -491,7 +490,7 @@ B200_API void b200_dtrie_destroy(b200_dtrie *);
  * account upserts / destructions, per-account slot upserts / deletions (zero value) / wipes.  Storage roots flow into the
  * account leaves on the device; only the touched paths of the touched tries are re-hashed.  This is the complete role
  * of reth's SparseStateTrie on the live path (crates/trie/sparse/src/state.rs) and of StateRoot::overlay_root_with_updates
- * (crates/trie/db/src/state.rs:184-230).  STATUS as b200_dtrie: emulation-validated, first B200 run pending.
+ * (crates/trie/db/src/state.rs:184-230).  STATUS as b200_dtrie (tests/test_gpu_dstate.py).
  *
  * create: like b200_state_root_full (segment a = storage of account a).
  * apply:  m account entries, keys strictly ascending; acct_flags[i]: bit 0 = exists after the block (0 = destroyed: its

@@ -1,4 +1,4 @@
-//! reth-trie-b200 — routes reth's state-commitment seams to the B200 engine.
+//! reth-trie-b200 — routes reth's state-commitment seams to the GPU engine (libb200trie.so).
 //!
 //! UNCOMPILED SKETCH (no Rust toolchain in the build image).  Seams (SURVEY.md §8b):
 //!   * `CustomStateRoot` closure   crates/engine/tree/src/tree/payload_validator.rs:2291-2310

@@ -5,7 +5,7 @@
  * link, import or call it; only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline /
  * --impl reference legs do.
  *
- * What it restates (reference paths relative to /root/reference):
+ * What it restates (reference paths relative to the root of the reth checkout):
  *   - keccak256                      alloy-primitives 1.6.0 `keccak256` (external crate; Keccak-f[1600],
  *                                    rate 136, pad 0x01..0x80) called from crates/trie/common/src/key.rs:4-18
  *   - HashBuilder / RLP / hex-prefix alloy-trie 0.9.5 `HashBuilder` (external crate), restated from its

@@ -1,6 +1,6 @@
-"""reth_b200 — B200-native state-root engine behind reth's StateRoot / StorageRoot / HashedPostState surface.
+"""reth_b200 — GPU state-root engine behind reth's StateRoot / StorageRoot / HashedPostState surface.
 
-The product is libb200trie.so (hand-written sm_100a CUDA behind the C ABI of include/b200trie.h); this
+The product is libb200trie.so (hand-written sm_90a CUDA for the H100 behind the C ABI of include/b200trie.h); this
 package is the host-side mirror of the reference interface used by tests and benchmarks.
 """
 from ._lib import B200Error, LIB_PATH  # noqa: F401

@@ -31,7 +31,7 @@
 
 using namespace b200;
 
-#define B200_VERSION_STR "reth_b200 0.2.0 (sm_100a)"
+#define B200_VERSION_STR "reth_b200 0.2.0 (sm_90a)"
 
 static thread_local int g_create_status = 0;
 

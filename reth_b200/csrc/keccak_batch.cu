@@ -127,7 +127,7 @@ static int sm_count() {
         int dev = 0;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&g_sm_count, cudaDevAttrMultiProcessorCount, dev);
-        if (g_sm_count <= 0) g_sm_count = 148;
+        if (g_sm_count <= 0) g_sm_count = 132;
     }
     return g_sm_count;
 }

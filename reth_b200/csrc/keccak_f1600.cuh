@@ -1,7 +1,7 @@
-// keccak_f1600.cuh — Keccak-f[1600] for sm_100a, one sponge per thread, state in registers.
+// keccak_f1600.cuh — Keccak-f[1600] for sm_90a, one sponge per thread, state in registers.
 //
-// Why thread-per-message and not a warp-cooperative layout: the permutation is ~122 LOP3 + ~58 SHF per round
-// on 32-bit halves (all on the ALU pipe: 64 lanes/clk/SM).  Spreading one state over 25 lanes of a warp turns
+// Why thread-per-message and not a warp-cooperative layout: the permutation is ~134 LOP3 + ~58 SHF per round
+// on 32-bit halves (sm_90a SASS, tools/sass_count.py) (all on the ALU pipe: 64 lanes/clk/SM).  Spreading one state over 25 lanes of a warp turns
 // every theta/pi/chi dependency into SHFL traffic (32 lanes/clk/SM, two SHFL per 64-bit lane) and idles 7/32
 // lanes; it is ~5x slower than keeping the 25 lanes in registers.  The warp-shuffle formulation survives where latency, not
 // throughput, is the bound: WarpKeccak in tk_warp.cuh (one warp per node for the sparse top levels of a trie and the dirty

@@ -338,9 +338,9 @@ __device__ __forceinline__ void thread_build_node(Strip<BLOCK> &s, uint32_t *sme
 
 // ------------------------------------------------------------------------------------------------ class 0, software-pipelined
 // The thread-per-node kernels gather through four dependent loads (node -> gap -> S/E -> meta/ref); ncu shows them stalled
-// on exactly that (long scoreboard 1.6 warps per issue slot at 3.5 resident warps per scheduler, ALU pipe 82 %).  For the
+// on exactly that (long-scoreboard stalls).  For the
 // class that holds most nodes (2 / 3 children, register path) the gather of node i+1 is therefore spread over the
-// permutation of node i: one level of the chain is issued after every six rounds, so every load has ~2 us of ALU work of
+// permutation of node i: one level of the chain is issued after every six rounds, so every load has six rounds of ALU work of
 // the same thread (and of its neighbours) in front of its first use.
 struct PrefetchedNode3 {
     uint32_t v, j0, k;      // node, first gap (sorted order), number of gaps (children - 1)

@@ -167,8 +167,8 @@ __global__ void partition_gather_kernel(const uint8_t *__restrict__ digests, con
     o[1] = q[1];
 }
 // out row i = in row perm[i], rows of `words` elements of T: one thread per element, so that a warp writes 32 consecutive
-// elements and reads runs of up to `words` consecutive ones (a row of 72 bytes = 9 x 8 bytes: 6 GB/s-class byte loops of a
-// thread-per-row copy took 2.5 ms for 5M rows, this takes the 0.15 ms the traffic costs)
+// elements and reads runs of up to `words` consecutive ones (a row of 72 bytes = 9 x 8 bytes; a thread-per-row byte loop
+// is many times slower than the traffic it moves)
 template <typename T>
 __global__ void gather_rows_kernel(const T *__restrict__ in, uint32_t words, const uint32_t *__restrict__ perm, uint64_t n,
                                    T *__restrict__ out) {

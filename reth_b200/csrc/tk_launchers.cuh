@@ -11,7 +11,7 @@ static int sms() {
         int dev = 0;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&g_sms, cudaDevAttrMultiProcessorCount, dev);
-        if (g_sms <= 0) g_sms = 148;
+        if (g_sms <= 0) g_sms = 132;
     }
     return g_sms;
 }

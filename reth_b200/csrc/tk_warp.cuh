@@ -4,7 +4,7 @@
 
 // ------------------------------------------------------------------------------------------------ warp-per-node
 // Small levels (the top of every trie, the dirty paths of an incremental update) hold too few nodes to fill the
-// machine; there the cost is the LATENCY of one node: 1-4 dependent Keccak-f on one thread is 20-40 us.  Here one
+// machine; there the cost is the LATENCY of one node: 1-4 dependent Keccak-f on one thread.  Here one
 // warp builds one node: the 16 child slots are assembled by 16 lanes in parallel, and the permutation runs with
 // the 25 lanes of the sponge state spread over 25 threads (theta/pi/chi as warp shuffles) — the layout the task
 // statement sketches.  It is ~5x less ALU-efficient than the register-resident sponge but ~5x shorter in latency,
@@ -101,7 +101,7 @@ __device__ __forceinline__ ChildInfo fetch_child_c(const ForestDev &f, uint32_t 
     return ci;
 }
 
-// (Same steps as the tail of warp_build_node below, which keeps its own copy: its SASS is the one measured on the B200.)
+// (Same steps as the tail of warp_build_node below, which keeps its own copy so that its SASS stays as measured.)
 // The assembled branch RLP (`total` bytes, padded into `blocks` rate blocks of `buf`) -> RlpNode of the node as seen from a
 // parent at depth pd: hashed if >= 32 bytes (or a trie root), wrapped in an extension node when more than one nibble
 // separates it from the parent.  Uniform control flow: all 32 lanes call.  Returns the meta byte (inline length | META_EXT).

@@ -1,4 +1,4 @@
-// trie_kernels.cu — level-synchronous Merkle-Patricia-Trie commitment on sm_100a.
+// trie_kernels.cu — level-synchronous Merkle-Patricia-Trie commitment on sm_90a.
 //
 // Replaces the serial stack machine of alloy-trie's HashBuilder (driven by StateRoot::calculate,
 // crates/trie/trie/src/trie.rs:247-309, and StorageRoot::calculate, :659-698) by a data-parallel

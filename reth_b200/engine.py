@@ -675,7 +675,7 @@ class ResidentTrie:
 class DynamicTrie:
     """Handle on a b200_dtrie: the account trie as an arena of 16-slot branch nodes in HBM; `apply` takes upserts and
     deletes in place and re-hashes only the touched paths (reth's sparse-trie role, crates/trie/sparse/src/parallel.rs).
-    Validated under tools/emu; first B200 run pending (see include/b200trie.h)."""
+    Validated against the oracle on the GPU (tests/test_gpu_dtrie.py) and under tools/emu."""
 
     def __init__(self, engine: Engine, handle, root: bytes):
         self.engine, self.handle, self._root = engine, handle, root
@@ -748,7 +748,7 @@ class DynamicTrie:
 
 class DynamicState:
     """Handle on a b200_dstate: accounts AND all storage tries resident; `apply` commits one block's hashed post state in
-    place (see include/b200trie.h).  Emulation-validated; first B200 run pending."""
+    place (see include/b200trie.h).  Validated against the oracle on the GPU (tests/test_gpu_dstate.py)."""
     EXISTS, UNCHANGED, WIPED = 1, 2, 4
 
     def __init__(self, engine: Engine, handle, root: bytes):

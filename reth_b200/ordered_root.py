@@ -1,4 +1,4 @@
-"""Host-side mirror of reth's ordered-root interface (crates/trie/common/src/ordered_root.rs) over the B200 engine.
+"""Host-side mirror of reth's ordered-root interface (crates/trie/common/src/ordered_root.rs) over the GPU engine.
 
 `OrderedTrieRootEncodedBuilder` keeps the reference's names, argument meaning and error behaviour (:146-257,
 `OrderedRootError` :9-80).  The reference flushes items into a HashBuilder as soon as the key order allows; here items

@@ -388,7 +388,7 @@ class DynamicStateRoot:
     (crates/trie/db/src/state.rs:184-230): `commit(HashedPostState)` applies one block in place — new / changed /
     destroyed accounts, slot writes, zeroed slots, wiped storages — and returns the new root with the block's
     `TrieUpdates` (account_nodes, removed_nodes, storage_tries with is_deleted).  Nothing of the state is kept on the host.
-    Emulation-validated; first B200 run pending (include/b200trie.h)."""
+    Validated against the oracle on the GPU (tests/test_gpu_dstate.py)."""
 
     def __init__(self, engine: Engine, state: HashedPostStateSorted, sharded: bool = False):
         """sharded=True: this object is one rank's shard (see reth_b200.sharded.ShardedDynamicStateRoot); `commit`'s root is

@@ -1,17 +1,18 @@
 #!/usr/bin/env python
 """Regenerates tests/golden/genesis_allocs.json from the reference's genesis files.
 
-Run in the build container only (/root/reference does not exist on the GPU box):
-    python tests/golden/make_fixtures.py
+Run against a checkout of reth (the tests only read the generated file):
+    python tests/golden/make_fixtures.py /path/to/reth
 
-Sources (data, not code): /root/reference/crates/chainspec/res/genesis/{mainnet,sepolia,holesky,goerli}.json
-(alloc + the `stateRoot` each file states) and /root/reference/crates/trie/trie/testdata/proof-genesis.json.
+Sources (data, not code): <reth>/crates/chainspec/res/genesis/{mainnet,sepolia,holesky,goerli}.json
+(alloc + the `stateRoot` each file states) and <reth>/crates/trie/trie/testdata/proof-genesis.json.
 Only the fields that enter the state root are kept: address -> balance, nonce, code, storage.
 """
 import json
 import os
+import sys
 
-REF = "/root/reference"
+REF = sys.argv[1] if len(sys.argv) > 1 else "."
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "genesis_allocs.json")
 
 

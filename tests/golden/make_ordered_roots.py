@@ -1,8 +1,8 @@
 """Generates tests/golden/ordered_roots.json from the reference's own ordered-root tests
 (crates/ethereum/primitives/src/receipt.rs:180-245: check_transaction_root, check_withdrawals_root,
-check_receipt_root_optimism).  Run in the build container, where /root/reference exists:
+check_receipt_root_optimism).  Run against a checkout of reth (the tests only read the generated file):
 
-    python tests/golden/make_ordered_roots.py
+    python tests/golden/make_ordered_roots.py /path/to/reth
 
 The block fixtures there are RLP blocks whose headers carry the expected roots; the items are the raw encodings found
 in the block body (what the encoder closure of ordered_trie_root_with_encoder writes for legacy transactions and
@@ -11,8 +11,10 @@ withdrawals).  The receipt case is assembled from the field values the test stat
 import json
 import os
 import re
+import sys
 
-SRC = "/root/reference/crates/ethereum/primitives/src/receipt.rs"
+REL = "crates/ethereum/primitives/src/receipt.rs"
+SRC = os.path.join(sys.argv[1] if len(sys.argv) > 1 else ".", REL)
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "ordered_roots.json")
 
 
@@ -108,7 +110,7 @@ def main():
     cases.append({"name": "check_receipt_root_optimism", "ref": "receipt.rs:218-244", "field": "receipts_root",
                   "items": [receipt.hex()], "root": root})
 
-    json.dump({"source": SRC.replace("/root/reference/", ""), "cases": cases}, open(OUT, "w"), indent=1)
+    json.dump({"source": REL, "cases": cases}, open(OUT, "w"), indent=1)
     print(f"wrote {OUT}: {len(cases)} cases")
 
 

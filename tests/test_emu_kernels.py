@@ -3,7 +3,7 @@ threads of a block, yield-based barriers and warp collectives), pass the fast pa
 bit-exact against the oracle and the golden vectors.
 
 This is a check of the *sources* (indexing, masks, RLP assembly, barrier placement), not a product path: only this
-test process points the loader at the emulated build (tests/conftest.py --emu); the B200 results come from the
+test process points the loader at the emulated build (tests/conftest.py --emu); the GPU results come from the
 `-m gpu` run of the very same tests on the real library."""
 import os
 import subprocess

@@ -220,7 +220,7 @@ def test_rejects_unsorted_or_duplicate_keys_and_stays_consistent(eng):
 
 def test_split_runs_share_an_attach_point(eng):
     """K1 < K2 < K3 where K1 and K3 diverge inside the (long) edge above a node N and K2 passes through it: K1 and K3 have the
-    same attach point without being neighbours in the sorted insert list.  The first B200 run caught this shape (two threads
+    same attach point without being neighbours in the sorted insert list.  The first GPU run caught this shape (two threads
     inserting at one attach word concurrently; sequential emulation could not see it): many such triples per block here."""
     rng = np.random.default_rng(31)
     state0 = {}

@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""Latency of the dynamic resident trie (b200_dtrie_*) on a B200 (a leg of bench.py).
+"""Latency of the dynamic resident trie (b200_dtrie_*) on the GPU (a leg of bench.py).
 
     python -m pytest tests/test_gpu_dtrie.py -m gpu -q      # correctness first
     python tools/dtrie_bench.py --base 100000000 --dirty 10000 --mix 80,10,10   # then latency
@@ -47,6 +47,7 @@ def main():
     accts[:, 40:72] = torch.frombuffer(bytearray(bytes.fromhex(
         "c5d2460186f7233c927e7db2dcc703c0e500b653ca82273b7bfad8045d85a470")), dtype=torch.uint8).to(dev)
     torch.cuda.synchronize()
+    torch.cuda.empty_cache()   # the generator's temporaries: the library allocates outside torch's cache
     t0 = time.perf_counter()
     trie = DynamicTrie.create_dev(eng, keys.view(torch.uint8).view(-1), accts.view(-1), None, n)
     torch.cuda.synchronize()
@@ -54,15 +55,20 @@ def main():
     note("dynamic trie created")
     ref = ResidentTrie.create_dev(eng, keys.view(torch.uint8).view(-1), accts.view(-1), None, n) if args.compare else None
     assert ref is None or trie.root() == ref.root()
+    # both tries hold their own copies of the inputs: keep host copies and hand the device memory back (two resident tries of
+    # 100M leaves and a merge + rebuild have to fit one 80 GB GPU)
+    base_keys_np = keys.view(torch.uint8).view(n, 32).cpu().numpy()
+    h_accts = accts.cpu().numpy().view(ACCOUNT_DTYPE).reshape(-1)
+    del keys, accts
+    torch.cuda.empty_cache()
     eng.set_stream(None)
     rng = np.random.default_rng(55)
-    live = keys.view(torch.uint8).view(n, 32).cpu().numpy()   # host copy of the key set, kept in step with the trie
+    live = base_keys_np.copy()   # host copy of the key set, kept in step with the trie
     live_set = None
     lat, dev_ms, built, mismatches, lat_rebuild, launches = [], [], [], 0, [], []
     base_root = trie.root()
     base_index = {}          # key -> row in the base arrays, for every key a block touched (the final undo block needs the base value)
     inserted_total = set()
-    h_accts = accts.cpu().numpy().view(ACCOUNT_DTYPE).reshape(-1)
     note("host copies ready")
     for b in range(args.blocks):
         note(f"block {b}")
@@ -105,7 +111,6 @@ def main():
     faulthandler.dump_traceback_later(240, exit=True)   # a hang below says where
     # ---- undo everything in one block: base values back, deleted base keys re-inserted, inserted keys deleted.  The root must
     # return to the root of the from-scratch build the trie was created from (independent of any model of the state).
-    base_keys_np = keys.view(torch.uint8).view(n, 32).cpu().numpy()
     # sorted with the keys; NATIVE byte order (searchsorted on a non-native array converts the whole array on every call)
     prefix = np.ascontiguousarray(base_keys_np[:, :8]).view(">u8").reshape(-1).astype(np.uint64)
 

@@ -56,7 +56,7 @@ unsigned cur = 0, block_threads = 0, alive = 0;
 unsigned bar_count = 0;
 uint64_t bar_gen = 0;
 bool in_kernel = false;
-alignas(128) unsigned char smem_buf[232448];  // 227 KB: the per-CTA maximum on sm_100
+alignas(128) unsigned char smem_buf[232448];  // 227 KB: the per-CTA maximum on sm_90
 }  // namespace
 }  // namespace emu
 

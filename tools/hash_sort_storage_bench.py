@@ -67,7 +67,7 @@ def main():
     h_sorted, h_perm = eng.pinned_empty((n, 64)), eng.pinned_empty((n,), np.uint32)
     eng.hash_sort_storage(h_addr, h_owner, h_slots, out=h_sorted, perm=h_perm)
     wall = []
-    for _ in range(max(3, args.reps // 2)):
+    for _ in range(args.reps):
         t0 = time.perf_counter()
         eng.hash_sort_storage(h_addr, h_owner, h_slots, out=h_sorted, perm=h_perm)
         wall.append((time.perf_counter() - t0) * 1e3)

@@ -43,7 +43,7 @@ def main():
     eng = Engine(0)
     roots = eng.ordered_roots(values, value_offsets, seg_offsets)  # warm-up (allocations)
     pageable = []
-    for _ in range(3):
+    for _ in range(args.reps):
         t0 = time.perf_counter()
         eng.ordered_roots(values, value_offsets, seg_offsets)
         pageable.append((time.perf_counter() - t0) * 1e3)

@@ -1,7 +1,7 @@
-// pipe_microbench.cu — issue-rate probes for the integer instructions Keccak-f is made of, on sm_100a.
+// pipe_microbench.cu — issue-rate probes for the integer instructions Keccak-f is made of, on sm_90a.
 // Answers: (1) LOP3 / SHF lanes per clock per SM (the ALU-pipe ceiling the keccak kernels are measured against),
 // (2) whether 64-bit rotations expressed as IMAD.WIDE / IMAD.HI (FMA pipe) can be co-issued with LOP3 so that
-// the rotation work leaves the ALU pipe.   Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 pipe_microbench.cu
+// the rotation work leaves the ALU pipe.   Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 pipe_microbench.cu
 #include <cstdint>
 #include <cstdio>
 #include <cuda_runtime.h>
@@ -119,8 +119,8 @@ void run(const char *name, int ops_per_acc, int sms, int warps_per_sm) {
     for (int i = 0; i < blocks; i++) avg += h[i];
     avg /= blocks;
     double ops_per_sm = (double)warps_per_sm * 32 * ITER * ACC * ops_per_acc;
-    printf("%-28s warps/SM=%2d  %7.1f lane-ops/clk/SM by clock64 | %7.1f by events at 1.965 GHz  (%.3f ms, clock64 rate %.3f GHz)  err=%s\n",
-           name, warps_per_sm, ops_per_sm / avg, ops_per_sm / (ms * 1e-3 * 1.965e9), ms, avg / (ms * 1e6),
+    printf("%-28s warps/SM=%2d  %7.1f lane-ops/clk/SM by clock64 | %7.1f by events at 1.98 GHz  (%.3f ms, clock64 rate %.3f GHz)  err=%s\n",
+           name, warps_per_sm, ops_per_sm / avg, ops_per_sm / (ms * 1e-3 * 1.98e9), ms, avg / (ms * 1e6),
            cudaGetErrorString(cudaGetLastError()));
     delete[] h;
     cudaFree(out);

@@ -1,9 +1,9 @@
 #!/usr/bin/env python3
 """ALU-pipe instructions per digest of keccak256_fixed32_kernel, counted from its SASS (the constant behind `alu_frac` in
-bench.py):   python tools/sass_count.py > profiles/r02_keccak_sass_count.txt
+bench.py):   python tools/sass_count.py
 The kernel is a grid-stride loop whose body is: loads + the peeled first round (`pre`), a 22-trip loop of one round each
 (`loop`), the peeled last round + stores (`post`).  LOP3 / SHF / ISETP / VIADD / LEA / IADD3 / SEL issue to the ALU pipe
-(64 lanes/clk/SM, profiles/r01_pipe_microbench.txt); IMAD / MOV go to the FMA pipe, LDG / STG to the LSU."""
+(64 lanes/clk/SM on compute capability 9.0); IMAD / MOV go to the FMA pipe, LDG / STG to the LSU."""
 import collections
 import os
 import subprocess
@@ -47,7 +47,7 @@ def main():
     print(f"  after it (peeled round 23, stores, loop control): {len(post)} instr, {n_alu(post)} ALU  {c(post)}")
     total, alu = len(pre) + 22 * len(loop) + len(post), n_alu(pre) + 22 * n_alu(loop) + n_alu(post)
     print(f"per digest: {total} instructions, {alu} on the ALU pipe")
-    print(f"ALU ceiling at 148 SMs x 64 lanes/clk x 1.965 GHz: {148 * 64 * 1.965e9 / alu / 1e9:.3f} G digests/s")
+    print(f"ALU ceiling per SM: {64 / alu * 1e3:.3f} digests per 1000 clocks (x 132 SMs x SM clock on an H100 SXM)")
 
 
 if __name__ == "__main__":

@@ -3,9 +3,9 @@
 
     python tools/sass_diff.py <git-rev>          # build <git-rev>'s reth_b200/csrc in /tmp and compare with the working tree
 
-Compiles both trees for sm_100a, dumps SASS with cuobjdump and compares every function of the OLD build instruction by
+Compiles both trees for sm_90a, dumps SASS with cuobjdump and compares every function of the OLD build instruction by
 instruction (opcodes, operands and encodings; addresses, -lineinfo comments and column padding ignored; anonymous-
-namespace name hashes normalised).  Used to show that kernels measured on the B200 are untouched by later work that
+namespace name hashes normalised).  Used to show that kernels measured on the GPU are untouched by later work that
 could only be checked under tools/emu."""
 import os
 import re
@@ -15,7 +15,7 @@ import tempfile
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 UNITS = ["trie_kernels", "keccak_batch", "hash_sort", "engine"]
-NVCC = ["nvcc", "-std=c++17", "-O3", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-Xcompiler",
+NVCC = ["nvcc", "-std=c++17", "-O3", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-Xcompiler",
         "-fPIC,-O3,-fvisibility=hidden"]
 
 

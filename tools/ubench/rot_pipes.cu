@@ -4,9 +4,8 @@
 // A rotate by r of the pair (lo, hi) is also  lo' = lo*2^r + hi32(hi*2^r),  hi' = hi*2^r + hi32(lo*2^r)  (the
 // two summands never share a bit), i.e. IMAD.HI + IMAD + IMAD.WIDE (with a 64-bit addend) on the FMA pipe.  The multipliers come from
 // constant memory so that ptxas cannot turn them back into shifts.  This bench times N permutations per thread
-// with K of the 29 rotates of every round moved over (K = 0: the shipping code).  Result (profiles/r02_rot_pipes.md): no gain,
-// the register-file operand bandwidth is shared by the two pipes.
-//   nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -o rot_pipes rot_pipes.cu && ./rot_pipes 64
+// with K of the 29 rotates of every round moved over (K = 0: the shipping code).
+//   nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -o rot_pipes rot_pipes.cu && ./rot_pipes 64
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
@@ -161,7 +160,7 @@ static void run(uint64_t *d_out, uint64_t *h_out, int blocks, int iters, uint64_
 }
 
 int main(int argc, char **argv) {
-    int blocks = 148 * 16 * 4, iters = 64;
+    int blocks = 132 * 16 * 4, iters = 64;  // 132 SMs (H100 SXM)
     if (argc > 1) iters = atoi(argv[1]);
     uint64_t *d_out, *h_out = (uint64_t *)malloc(1024 * 8);
     cudaMalloc(&d_out, (size_t)blocks * 128 * 8);
