@@ -4,7 +4,7 @@
 //
 // Layout: message i at in + i*stride, digest i at out + 32*i.  One message per thread, sponge state in
 // registers, grid-stride loop over a persistent grid (SM count x resident CTAs).  Algorithmic traffic is
-// msg_len + 32 bytes per digest; the kernel is ALU-bound (one Keccak-f = ~4.3k LOP3/SHF), not HBM-bound.
+// msg_len + 32 bytes per digest; the kernel is ALU-bound (one Keccak-f = ~4.2k LOP3/SHF), not HBM-bound.
 #include "keccak_f1600.cuh"
 #include "kernels.h"
 

@@ -1,6 +1,6 @@
 // keccak_f1600.cuh — Keccak-f[1600] for sm_90a, one sponge per thread, state in registers.
 //
-// Why thread-per-message and not a warp-cooperative layout: the permutation is ~134 LOP3 + ~58 SHF per round
+// Why thread-per-message and not a warp-cooperative layout: the permutation is 122 LOP3 + 58 SHF per round
 // on 32-bit halves (sm_90a SASS, tools/sass_count.py) (all on the ALU pipe: 64 lanes/clk/SM).  Spreading one state over 25 lanes of a warp turns
 // every theta/pi/chi dependency into SHFL traffic (32 lanes/clk/SM, two SHFL per 64-bit lane) and idles 7/32
 // lanes; it is ~5x slower than keeping the 25 lanes in registers.  The warp-shuffle formulation survives where latency, not
@@ -41,16 +41,43 @@ __device__ __forceinline__ uint64_t rotl64(uint64_t x) {
     return ((uint64_t)nhi << 32) | nlo;
 }
 
-// One round: theta, rho, pi, chi, iota.  Written so that nothing moves: pi is pure renaming.
+// a ^ b ^ c as one three-input LOP3 (LUT 0x96) per 32-bit half.  Written out because ptxas for sm_90a re-factors
+// theta: from `a[i] ^ c[x-1] ^ rotl1(c[x+1])` it hoists the common D[x] = c[x-1] ^ rotl1(c[x+1]) and then spends one
+// two-input XOR per lane half on a[i] ^ D[x] (10 + 50 LOP3 per round instead of 50), and it splits the five-way
+// column parities the same way.  Inline PTX is kept as written.  The asm is not volatile, so lanes whose result is
+// dead (the last round of a squeeze) are still removed.  The plain C++ form serves host compilers (tools/emu) and
+// rounds whose state holds compile-time zeros (PLAIN = true), which the compiler can only fold through plain XORs.
+// One asm statement on 64-bit operands rather than one per half: with the latter, ptxas changed how it compiled
+// unrelated code of the strip-based kernels (branch_kernel<128,16> and wavefront_thread_kernel<64> grew 4-5x).
+template <bool PLAIN = false>
+__device__ __forceinline__ uint64_t xor3(uint64_t a, uint64_t b, uint64_t c) {
+#ifdef __CUDA_ARCH__
+    if constexpr (!PLAIN) {
+        uint64_t r;
+        asm("{\n\t.reg .b32 al, ah, bl, bh, cl, ch, rl, rh;\n\t"
+            "mov.b64 {al, ah}, %1;\n\tmov.b64 {bl, bh}, %2;\n\tmov.b64 {cl, ch}, %3;\n\t"
+            "lop3.b32 rl, al, bl, cl, 0x96;\n\tlop3.b32 rh, ah, bh, ch, 0x96;\n\t"
+            "mov.b64 %0, {rl, rh};\n\t}"
+            : "=l"(r) : "l"(a), "l"(b), "l"(c));
+        return r;
+    }
+#endif
+    return a ^ b ^ c;
+}
+
+// One round: theta, rho, pi, chi, iota.  Written so that nothing moves: pi is pure renaming.  Per round on 32-bit
+// halves: 20 LOP3 for the column parities, 50 for theta, 50 for chi, 1-2 for iota, 58 SHF for the rotations.
+// PLAIN: see xor3 (the peeled first round of a single-block short message, where 20 lanes are zero).
+template <bool PLAIN = false>
 __device__ __forceinline__ void keccak_round(uint64_t (&a)[25], uint64_t rc) {
-    uint64_t c0 = a[0] ^ a[5] ^ a[10] ^ a[15] ^ a[20];
-    uint64_t c1 = a[1] ^ a[6] ^ a[11] ^ a[16] ^ a[21];
-    uint64_t c2 = a[2] ^ a[7] ^ a[12] ^ a[17] ^ a[22];
-    uint64_t c3 = a[3] ^ a[8] ^ a[13] ^ a[18] ^ a[23];
-    uint64_t c4 = a[4] ^ a[9] ^ a[14] ^ a[19] ^ a[24];
+    uint64_t c0 = xor3<PLAIN>(xor3<PLAIN>(a[0], a[5], a[10]), a[15], a[20]);
+    uint64_t c1 = xor3<PLAIN>(xor3<PLAIN>(a[1], a[6], a[11]), a[16], a[21]);
+    uint64_t c2 = xor3<PLAIN>(xor3<PLAIN>(a[2], a[7], a[12]), a[17], a[22]);
+    uint64_t c3 = xor3<PLAIN>(xor3<PLAIN>(a[3], a[8], a[13]), a[18], a[23]);
+    uint64_t c4 = xor3<PLAIN>(xor3<PLAIN>(a[4], a[9], a[14]), a[19], a[24]);
     // d[x] = c[x-1] ^ rotl(c[x+1],1); folded into the 3-input xor below so that theta costs one LOP3 per half
     uint64_t r0 = rotl64<1>(c1), r1 = rotl64<1>(c2), r2 = rotl64<1>(c3), r3 = rotl64<1>(c4), r4 = rotl64<1>(c0);
-#define TH(i, cm, rp) (a[i] ^ cm ^ rp)
+#define TH(i, cm, rp) xor3<PLAIN>(a[i], cm, rp)
     uint64_t b00 = TH(0, c4, r0);
     uint64_t b10 = rotl64<1>(TH(1, c0, r1));
     uint64_t b20 = rotl64<62>(TH(2, c1, r2));
@@ -125,10 +152,13 @@ __device__ __forceinline__ void keccak_rounds(uint64_t (&a)[25]) {
     for (int r = R0; r < R1; r++) keccak_round(a, KECCAK_RC[r]);
 }
 
-// Single-block message whose state is mostly compile-time zeros (a 20/32-byte key): round 0 is peeled too, so
-// that the compiler folds the XORs with the 20 zero lanes and the constant pad lanes.
+// Single-block message whose state is mostly compile-time zeros (a 20/32-byte key): round 0 is peeled too, and
+// written with plain XORs, so that the compiler folds the XORs with the 20 zero lanes and the constant pad lanes.
+// Rounds 1..22 stay a loop: unrolled in line with immediate round constants they are 2 % fewer ALU instructions
+// (4141 against 4217 per digest) but ~67 KB of code, and keccak256_fixed32_kernel ran 14 % slower that way
+// (3.41 against 3.91-3.98 G digests/s on one H100 SXM, 400 W), presumably limited by instruction fetch (not profiled).
 __device__ __forceinline__ void keccak_f1600_sparse_final(uint64_t (&a)[25]) {
-    keccak_round(a, 0x0000000000000001ULL);
+    keccak_round<true>(a, 0x0000000000000001ULL);
 #pragma unroll 1
     for (int r = 1; r < 23; r++) keccak_round(a, KECCAK_RC[r]);
     keccak_round(a, 0x8000000080008008ULL);

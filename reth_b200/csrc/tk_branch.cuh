@@ -183,7 +183,7 @@ __device__ __forceinline__ uint32_t encode_branch_u(Strip<BLOCK> &s, const Fores
                 s.byte(0xa0);
                 s.words8(ref);
             } else {
-                for (uint32_t b = 0; b < clen; b++) s.byte(byte_at(ref, b));
+                s.head32(ref, clen);
             }
             cur++;
         }

@@ -53,6 +53,17 @@ struct Strip {
             }
         }
     }
+    // bytes [0, len) of a 32-byte string held as 8 little-endian words (an inline child reference, len < 32): whole
+    // words, then the 0..3 bytes of the partial one.  Every word index is a constant, so the string stays in registers.
+    __device__ __forceinline__ void head32(const uint32_t (&x)[8], uint32_t len) {
+        uint32_t part = 0;
+#pragma unroll
+        for (int i = 0; i < 8; i++) {
+            if (4u * i + 4 <= len) word(x[i]);
+            else if (4u * i < len) part = x[i];
+        }
+        for (uint32_t b = 0; b < (len & 3); b++) byte((part >> (8 * b)) & 0xff);
+    }
     __device__ __forceinline__ uint32_t length() const { return nw * 4 + nb; }
     __device__ __forceinline__ uint32_t read_word(uint32_t i) const { return w[i * BLOCK]; }
     // Keccak pad10*1 to a multiple of the 136-byte rate; returns the number of rate blocks.
