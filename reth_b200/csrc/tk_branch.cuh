@@ -9,6 +9,8 @@ struct ChildInfo {
     uint32_t meta;  // low 5 bits inline length (0 = hashed), META_EXT, META_STORED
 };
 
+// COHERENT: loads that bypass L1 (data produced by other SMs earlier in the SAME kernel: the wavefront)
+template <bool COHERENT = false>
 __device__ __forceinline__ ChildInfo fetch_child(const ForestDev &f, uint32_t j0, uint32_t c) {
     ChildInfo ci;
     if (c == 0) {
@@ -20,7 +22,8 @@ __device__ __forceinline__ ChildInfo fetch_child(const ForestDev &f, uint32_t j0
         ci.id = f.S[g];
         ci.nib = f.nibs[g] & 15;
     }
-    ci.meta = ci.id < f.n ? f.leaf_meta[ci.id] : f.node_meta[ci.id - (uint32_t)f.n];
+    if (COHERENT) ci.meta = ci.id < f.n ? __ldcg(f.leaf_meta + ci.id) : __ldcg(f.node_meta + (ci.id - (uint32_t)f.n));
+    else ci.meta = ci.id < f.n ? f.leaf_meta[ci.id] : f.node_meta[ci.id - (uint32_t)f.n];
     return ci;
 }
 
@@ -41,54 +44,6 @@ __device__ __forceinline__ uint32_t put_ext_path(W &s, const uint8_t *key, uint3
     return hp_len == 1 ? 1 : 1 + hp_len;
 }
 
-// Builds branch node v (depth d) into the strip; returns RLP length and the node's masks / extent.
-template <int BLOCK>
-__device__ __forceinline__ uint32_t encode_branch(Strip<BLOCK> &s, const ForestDev &f, uint32_t j0, uint32_t k,
-                                                  uint32_t &state_mask, uint32_t &tree_mask, uint32_t &hash_mask,
-                                                  uint32_t &l, uint32_t &r) {
-    // pass 1: lengths and masks
-    uint32_t payload = 17;
-    state_mask = tree_mask = hash_mask = 0;
-    for (uint32_t c = 0; c <= k; c++) {
-        ChildInfo ci = fetch_child(f, j0, c);
-        uint32_t clen = (ci.meta & META_LEN) ? (ci.meta & META_LEN) : 33;
-        payload += clen - 1;
-        uint32_t bit = 1u << ci.nib;
-        state_mask |= bit;
-        if (ci.id >= f.n || (ci.meta & META_ISNODE)) {
-            if (!(ci.meta & META_EXT)) {
-                hash_mask |= bit;
-                if ((ci.meta & META_LEN) && f.retain_updates) atomicExch(f.err, B200_DEVERR_INLINE_HASH_CHILD);
-            }
-            if (ci.meta & META_STORED) tree_mask |= bit;
-        }
-        if (c == 0) l = ci.id < f.n ? ci.id : f.node_l[ci.id - (uint32_t)f.n];
-        if (c == k) r = ci.id < f.n ? ci.id : f.node_r[ci.id - (uint32_t)f.n];
-    }
-    // pass 2: bytes
-    put_list_header(s, payload);
-    uint32_t cur = 0;
-    for (uint32_t c = 0; c <= k; c++) {
-        ChildInfo ci = fetch_child(f, j0, c);
-        for (; cur < ci.nib; cur++) s.byte(0x80);
-        const uint8_t *rp = ci.id < f.n ? f.leaf_ref + 32 * (uint64_t)ci.id
-                                        : f.node_ref + 32 * (uint64_t)(ci.id - (uint32_t)f.n);
-        uint32_t ref[8];
-        load32_nc(rp, ref);
-        uint32_t clen = ci.meta & META_LEN;
-        if (clen == 0) {
-            s.byte(0xa0);
-            s.words8(ref);
-        } else {
-            for (uint32_t b = 0; b < clen; b++) s.byte(byte_at(ref, b));
-        }
-        cur++;
-    }
-    for (; cur < 16; cur++) s.byte(0x80);
-    s.byte(0x80);  // value slot
-    return list_header_len(payload) + payload;
-}
-
 // Wraps `child` (ref words + inline length, 0 = hashed) into an extension over key nibbles [from,to).
 template <class W>
 __device__ __forceinline__ uint32_t encode_extension(W &s, const uint8_t *key, uint32_t from, uint32_t to,
@@ -100,18 +55,14 @@ __device__ __forceinline__ uint32_t encode_extension(W &s, const uint8_t *key, u
     uint32_t payload = path_str + clen;
     put_list_header(s, payload);
     put_ext_path(s, key, from, to);
-    if (child_inline_len == 0) {
-        s.byte(0xa0);
-        s.words8(child);
-    } else {
-        for (uint32_t b = 0; b < child_inline_len; b++) s.byte(byte_at(child, b));
-    }
+    put_child(s, child, child_inline_len);
     return list_header_len(payload) + payload;
 }
 
-// Class-specialised variant of encode_branch: at most MAXC children, every per-child quantity lives in registers
-// and all the dependent global loads of a phase (gap -> S/E -> meta -> ref) are issued back to back for the
-// whole node before any of them is consumed, so one thread keeps up to MAXC requests in flight.
+// Builds the branch node over gaps [j0, j0 + k) into the strip; returns its RLP length and the node's masks / extent.
+// At most MAXC children: every per-child quantity lives in registers and all the dependent global loads of a phase
+// (gap -> S/E -> meta -> ref) are issued back to back for the whole node before any of them is consumed, so one
+// thread keeps up to MAXC requests in flight.
 template <int BLOCK, int MAXC, bool COHERENT = false>
 __device__ __forceinline__ uint32_t encode_branch_u(Strip<BLOCK> &s, const ForestDev &f, uint32_t j0, uint32_t k,
                                                     uint32_t &state_mask, uint32_t &tree_mask, uint32_t &hash_mask,
@@ -167,24 +118,12 @@ __device__ __forceinline__ uint32_t encode_branch_u(Strip<BLOCK> &s, const Fores
         if ((uint32_t)c <= k) {
             const uint8_t *rp = id[c] < n ? f.leaf_ref + 32 * (uint64_t)id[c] : f.node_ref + 32 * (uint64_t)(id[c] - n);
             uint32_t ref[8];
-            if (COHERENT) {
-                const uint4 *q = reinterpret_cast<const uint4 *>(rp);
-                uint4 x = __ldcg(q), y = __ldcg(q + 1);
-                ref[0] = x.x; ref[1] = x.y; ref[2] = x.z; ref[3] = x.w;
-                ref[4] = y.x; ref[5] = y.y; ref[6] = y.z; ref[7] = y.w;
-            } else {
-                load32_nc(rp, ref);
-            }
+            if (COHERENT) load32_cg(rp, ref);
+            else load32_nc(rp, ref);
             uint32_t nibble = nm[c] & 15;
             s.fill80(nibble - cur);
             cur = nibble;
-            uint32_t clen = (nm[c] >> 8) & META_LEN;
-            if (clen == 0) {
-                s.byte(0xa0);
-                s.words8(ref);
-            } else {
-                s.head32(ref, clen);
-            }
+            put_child(s, ref, (nm[c] >> 8) & META_LEN);
             cur++;
         }
     }
@@ -244,6 +183,19 @@ __device__ __forceinline__ void branch23_words(const uint32_t (&r0)[8], const ui
     xor_child33(m, 0, r0, n0, true);
     xor_child33(m, 8, r1, n1, true);
     xor_child33(m, 16, r2, n2, three);
+}
+
+// The reference (ref, meta) of a node of depth d as seen from its parent at depth pd: wrapped into an extension node over
+// key nibbles [pd + 1, d) when more than one nibble separates the two (through the strip, which the node's own RLP no
+// longer needs).  Returns the new meta.
+template <int BLOCK>
+__device__ __forceinline__ uint32_t thread_finish_node(Strip<BLOCK> &s, uint32_t (&ref)[8], uint32_t meta, int pd, int d,
+                                                       const uint8_t *key, uint32_t &hashed, uint32_t &exts) {
+    if (pd + 1 >= d) return meta;
+    s.reset();
+    uint32_t elen = encode_extension(s, key, (uint32_t)(pd + 1), (uint32_t)d, ref, meta);
+    exts++;
+    return strip_to_ref(s, elen, pd < 0, ref, hashed) | META_EXT;
 }
 
 // One thread builds branch node v of depth d into its strip, hashes it and publishes it (node arrays, S/E).
@@ -308,22 +260,11 @@ __device__ __forceinline__ void thread_build_node(Strip<BLOCK> &s, uint32_t *sme
             done = true;
         }
     }
-    if (!done) {
-        uint32_t len = encode_branch_u<BLOCK, MAXC, COHERENT>(s, f, j0, k, state_mask, tree_mask, hash_mask, l, r);
-        int pdl0 = depth_of(f.Lp[l]), pdr0 = depth_of(f.Lp[(uint64_t)r + 1]);
-        int pd0 = pdl0 > pdr0 ? pdl0 : pdr0;
-        meta = strip_to_ref(s, len, pd0 < 0 && !(pd0 + 1 < d), ref, hashed);
-    }
-    int pdl = depth_of(f.Lp[l]), pdr = depth_of(f.Lp[(uint64_t)r + 1]);
-    int pd = pdl > pdr ? pdl : pdr;
-    bool is_root = pd < 0;
-    bool need_ext = pd + 1 < d;
-    if (need_ext) {
-        s.reset();
-        uint32_t elen = encode_extension(s, f.keys + 32 * (uint64_t)l, (uint32_t)(pd + 1), (uint32_t)d, ref, meta);
-        meta = strip_to_ref(s, elen, is_root, ref, hashed) | META_EXT;
-        exts++;
-    }
+    uint32_t len = 0;
+    if (!done) len = encode_branch_u<BLOCK, MAXC, COHERENT>(s, f, j0, k, state_mask, tree_mask, hash_mask, l, r);
+    const int pd = parent_depth(f, l, r);
+    if (!done) meta = strip_to_ref(s, len, pd < 0 && pd + 1 >= d, ref, hashed);
+    meta = thread_finish_node(s, ref, meta, pd, d, f.keys + 32 * (uint64_t)l, hashed, exts);
     bool stored = (tree_mask | hash_mask) != 0;
     if (stored) meta |= META_STORED;
     store32(f.node_ref + 32 * (uint64_t)v, ref);
@@ -398,6 +339,7 @@ __global__ void __launch_bounds__(BLOCK, 4) branch3_pipelined_kernel(ForestDev f
     extern __shared__ uint32_t smem[];
     if (*(volatile int *)f.err != B200_DEVERR_NONE) return;
     Strip<BLOCK> s;
+    s.init(smem);
     uint32_t hashed = 0, exts = 0;
     const uint32_t step = gridDim.x * BLOCK;
     const uint32_t n = (uint32_t)f.n;
@@ -452,12 +394,7 @@ __global__ void __launch_bounds__(BLOCK, 4) branch3_pipelined_kernel(ForestDev f
             hashed++;
             int pdl = depth_of(lpl), pdr = depth_of(lpr);
             int pd = pdl > pdr ? pdl : pdr;
-            if (pd + 1 < d) {  // extension node above the branch (rare for hashed keys): through the strip
-                s.init(smem);
-                uint32_t elen = encode_extension(s, f.keys + 32 * (uint64_t)l, (uint32_t)(pd + 1), (uint32_t)d, ref, 0u);
-                meta = strip_to_ref(s, elen, pd < 0, ref, hashed) | META_EXT;
-                exts++;
-            }
+            meta = thread_finish_node(s, ref, 0u, pd, d, f.keys + 32 * (uint64_t)l, hashed, exts);  // rare for hashed keys
             if ((tree_mask | hash_mask) != 0) meta |= META_STORED;
             store32(f.node_ref + 32 * (uint64_t)v, ref);
             f.node_meta[v] = (uint8_t)meta;
@@ -476,14 +413,7 @@ __global__ void __launch_bounds__(BLOCK, 4) branch3_pipelined_kernel(ForestDev f
         cur = nx;
         p += step;
     }
-    for (int o = 16; o; o >>= 1) {
-        hashed += __shfl_xor_sync(0xffffffffu, hashed, o);
-        exts += __shfl_xor_sync(0xffffffffu, exts, o);
-    }
-    if ((threadIdx.x & 31) == 0) {
-        if (hashed) atomicAdd(&f.counters[CNT_HASHED], (unsigned long long)hashed);
-        if (exts) atomicAdd(&f.counters[CNT_EXT], (unsigned long long)exts);
-    }
+    flush_counters(f.counters, hashed, exts);
 }
 
 // One thread per branch node of depth d.  MAXC bounds the children of every node in [pos_lo, pos_hi) (the level's
@@ -500,12 +430,5 @@ __global__ void __launch_bounds__(BLOCK) branch_kernel(ForestDev f, const uint32
         uint32_t ref[8];
         thread_build_node<BLOCK, MAXC, false>(s, smem, f, __ldg(node_order + p64), d, hashed, exts, ref);
     }
-    for (int o = 16; o; o >>= 1) {
-        hashed += __shfl_xor_sync(0xffffffffu, hashed, o);
-        exts += __shfl_xor_sync(0xffffffffu, exts, o);
-    }
-    if ((threadIdx.x & 31) == 0) {
-        if (hashed) atomicAdd(&f.counters[CNT_HASHED], (unsigned long long)hashed);
-        if (exts) atomicAdd(&f.counters[CNT_EXT], (unsigned long long)exts);
-    }
+    flush_counters(f.counters, hashed, exts);
 }

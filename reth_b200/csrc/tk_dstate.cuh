@@ -16,7 +16,6 @@ __global__ void __launch_bounds__(512) dt_frontier_kernel(DTrieDev t, const uint
     __shared__ __align__(16) uint8_t sbuf[16][WARP_BUF];
     const int lane = threadIdx.x & 31, b = threadIdx.x >> 5;
     uint8_t *buf = sbuf[b];
-    uint32_t *bufw = reinterpret_cast<uint32_t *>(buf);
     WarpKeccak kw;
     kw.init(lane);
     FrontierEntryDev &e = out[b];
@@ -27,42 +26,17 @@ __global__ void __launch_bounds__(512) dt_frontier_kernel(DTrieDev t, const uint
     uint32_t out8[8], hashed = 0, exts = 0, meta;
     if (w & DT_LEAF) {
         const uint32_t x = w & ~DT_LEAF;
-        for (uint32_t q = lane; q < 68; q += 32) bufw[q] = 0;
-        __syncwarp();
-        uint32_t len = 0;
-        if (lane == 0) {
-            uint32_t k[8];
-            load32_nc(t.lkey + 32 * (uint64_t)x, k);
-            LinBuf lb{buf, 0};
-            len = encode_leaf<LinBuf, true>(lb, k, 0, t.lval + 72 * (uint64_t)x, t.lsroot ? t.lsroot + 32 * (uint64_t)x : nullptr, t.err);
-            buf[len] |= 0x01;
-            buf[(len / 136 + 1) * 136 - 1] |= 0x80;
-        }
-        len = __shfl_sync(0xffffffffu, len, 0);
-        __syncwarp();
-        uint64_t a = kw.hash(buf, len / 136 + 1, lane);  // account leaves are >= 70 bytes: always a hash reference
-#pragma unroll
-        for (int q = 0; q < 4; q++) {
-            uint64_t v = shfl64(a, q);
-            out8[2 * q] = (uint32_t)v;
-            out8[2 * q + 1] = (uint32_t)(v >> 32);
-        }
-        meta = 0;
+        meta = warp_leaf_ref(true, buf, t.lkey + 32 * (uint64_t)x, 0, t.lval + 72 * (uint64_t)x,
+                             t.lsroot ? t.lsroot + 32 * (uint64_t)x : nullptr, t.err, kw, lane, hashed, out8);
     } else {
         meta = dt_warp_build_node<0>(t, w, buf, kw, lane, hashed, exts, out8);
     }
     if (lane == 0) {
         e.as_root_len = 32;
         for (int i = 0; i < 32; i++) e.as_root[i] = bucket_roots[32 * b + i];
-        uint32_t il = meta & META_LEN;
-        if (il == 0) {
-            e.as_child_len = 33;
-            e.as_child[0] = 0xa0;
-            for (int i = 0; i < 32; i++) e.as_child[1 + i] = (uint8_t)(out8[i >> 2] >> (8 * (i & 3)));
-        } else {
-            e.as_child_len = (uint8_t)il;
-            for (uint32_t i = 0; i < il; i++) e.as_child[i] = (uint8_t)(out8[i >> 2] >> (8 * (i & 3)));
-        }
+        LinBuf lb{e.as_child, 0};
+        put_child(lb, out8, meta & META_LEN);
+        e.as_child_len = (uint8_t)lb.n;
     }
 }
 

@@ -689,6 +689,65 @@ __global__ void __launch_bounds__(BLOCK) dt_restructure_fused_kernel(DTrieDev t,
     for (uint32_t e = tid; e < n_seeds; e += BLOCK) dt_starts_entry(t, e);
 }
 
+// ------------------------------------------------------------------------------------------------ node encoding
+// Payload length of the RLP of node v (16 child slots + the empty value slot) and its masks.  COHERENT: loads that
+// bypass L1 (the wavefronts read what other SMs wrote earlier in the same kernel).
+template <bool COHERENT>
+static __device__ __forceinline__ uint32_t dt_branch_payload(const DTrieDev &t, uint32_t v, uint32_t &state_mask,
+                                                            uint32_t &tree_mask, uint32_t &hash_mask) {
+    const uint32_t *ch = t.nchild + 16 * (uint64_t)v;
+    uint32_t payload = 1;
+    state_mask = tree_mask = hash_mask = 0;
+    for (int k = 0; k < 16; k++) {
+        uint32_t cw = ch[k];
+        if (cw == DT_NONE) {
+            payload += 1;
+            continue;
+        }
+        bool leaf = (cw & DT_LEAF) != 0;
+        const uint8_t *mp = leaf ? t.lmeta + (cw & ~DT_LEAF) : t.nmeta + cw;
+        uint32_t m = COHERENT ? __ldcg(mp) : *mp;
+        payload += (m & META_LEN) ? (m & META_LEN) : 33u;
+        state_mask |= 1u << k;
+        if (!leaf) {
+            if (!(m & META_EXT)) {
+                hash_mask |= 1u << k;
+                if (COHERENT && (m & META_LEN)) atomicExch(t.err, B200_DEVERR_INLINE_HASH_CHILD);  // builders only
+            }
+            if (m & META_STORED) tree_mask |= 1u << k;
+        }
+    }
+    return payload;
+}
+// The RLP of node v, given its payload length
+template <bool COHERENT, class W>
+static __device__ __forceinline__ void dt_put_branch(W &s, const DTrieDev &t, uint32_t v, uint32_t payload) {
+    const uint32_t *ch = t.nchild + 16 * (uint64_t)v;
+    put_list_header(s, payload);
+    for (int k = 0; k < 16; k++) {
+        uint32_t cw = ch[k];
+        if (cw == DT_NONE) {
+            s.byte(0x80);
+            continue;
+        }
+        bool leaf = (cw & DT_LEAF) != 0;
+        uint32_t id = cw & ~DT_LEAF;
+        const uint8_t *mp = leaf ? t.lmeta + id : t.nmeta + id;
+        const uint8_t *rp = (leaf ? t.lref : t.nref) + 32 * (uint64_t)id;
+        uint32_t ref[8];
+        if (COHERENT) load32_cg(rp, ref);
+        else load32_nc(rp, ref);
+        const uint32_t il = (COHERENT ? __ldcg(mp) : *mp) & META_LEN;
+        if (il == 0) {
+            s.byte(0xa0);
+            s.words8(ref);
+        } else {  // (not put_child: with it, ptxas keeps the leaf arrays of dt_wavefront_thread_kernel in local memory)
+            for (uint32_t b = 0; b < il; b++) s.byte(byte_at(ref, b));
+        }
+    }
+    s.byte(0x80);
+}
+
 // One warp builds node v from its 16 child slots (lane = nibble).  All 32 lanes must call.
 // PD_OVERRIDE >= -1: encode as if the parent were at that depth and leave the arena untouched (multi-GPU frontier:
 // a bucket's top node as child of the depth-0 root branch); returns the RlpNode meta (inline length | META_EXT ...).
@@ -705,10 +764,7 @@ __device__ __forceinline__ uint32_t dt_warp_build_node(const DTrieDev &t, uint32
     uint32_t cmeta = 0;
     if (has) {
         cmeta = __ldcg(is_leaf ? t.lmeta + id : t.nmeta + id);
-        const uint4 *q = reinterpret_cast<const uint4 *>((is_leaf ? t.lref : t.nref) + 32 * (uint64_t)id);
-        uint4 x = __ldcg(q), y = __ldcg(q + 1);
-        ref[0] = x.x; ref[1] = x.y; ref[2] = x.z; ref[3] = x.w;
-        ref[4] = y.x; ref[5] = y.y; ref[6] = y.z; ref[7] = y.w;
+        load32_cg((is_leaf ? t.lref : t.nref) + 32 * (uint64_t)id, ref);
     }
     const uint32_t clen = lane < 16 ? (has ? ((cmeta & META_LEN) ? (cmeta & META_LEN) : 33u) : 1u) : 0u;
     const uint32_t bit = has ? (1u << lane) : 0u;
@@ -735,21 +791,9 @@ __device__ __forceinline__ uint32_t dt_warp_build_node(const DTrieDev &t, uint32
         put_list_header(lb, payload);
     }
     if (lane < 16) {
-        uint32_t off = hdr + incl - clen;
-        if (!has) {
-            buf[off] = 0x80;
-        } else if ((cmeta & META_LEN) == 0) {
-            buf[off++] = 0xa0;
-#pragma unroll
-            for (int i = 0; i < 8; i++) {
-                buf[off++] = (uint8_t)ref[i];
-                buf[off++] = (uint8_t)(ref[i] >> 8);
-                buf[off++] = (uint8_t)(ref[i] >> 16);
-                buf[off++] = (uint8_t)(ref[i] >> 24);
-            }
-        } else {
-            for (uint32_t b = 0; b < clen; b++) buf[off++] = (uint8_t)byte_at(ref, b);
-        }
+        LinBuf lb{buf + hdr + incl - clen, 0};
+        if (has) put_child(lb, ref, cmeta & META_LEN);
+        else lb.byte(0x80);
     }
     if (lane == 16) {
         buf[total - 1] = 0x80;
@@ -777,6 +821,28 @@ __device__ __forceinline__ uint32_t dt_warp_build_node(const DTrieDev &t, uint32
     return meta;
 }
 
+// The last-arriver climb of a warp from node p (see warp_climb); true iff this warp re-hashed the root of its trie.
+static __device__ __forceinline__ bool dt_warp_climb(const DTrieDev &t, uint32_t p, uint8_t *buf, const WarpKeccak &kw, int lane,
+                                                     uint32_t &hashed, uint32_t &exts, uint32_t (&out)[8]) {
+    for (int hops = 0; p != DT_NONE; hops++) {
+        if (hops > DT_MAX_HOPS) {  // uniform across the warp
+            if (lane == 0) atomicExch(t.err, B200_DEVERR_CORRUPT);
+            return false;
+        }
+        uint32_t last = 0;
+        if (lane == 0) {
+            __threadfence();
+            last = atomicSub(&t.npending[p], 1u) == 1u;
+            __threadfence();
+        }
+        last = __shfl_sync(0xffffffffu, last, 0);
+        if (!last) return false;
+        dt_warp_build_node(t, p, buf, kw, lane, hashed, exts, out);
+        p = t.nparent[p];
+    }
+    return true;
+}
+
 // One warp per seed: re-hash the item if nothing below it is dirty, then climb; the last dirty child to arrive at a
 // node re-hashes it.  The warp that runs out of parents holds the new root reference.
 template <int WARPS>
@@ -785,7 +851,6 @@ __global__ void __launch_bounds__(WARPS * 32) dt_wavefront_kernel(DTrieDev t, co
     if (*(volatile int *)t.err != B200_DEVERR_NONE) return;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     uint8_t *buf = sbuf[warp];
-    uint32_t *bufw = reinterpret_cast<uint32_t *>(buf);
     WarpKeccak kw;
     kw.init(lane);
     uint32_t hashed = 0, exts = 0;
@@ -797,80 +862,24 @@ __global__ void __launch_bounds__(WARPS * 32) dt_wavefront_kernel(DTrieDev t, co
         uint32_t p;
         if (s & DT_LEAF) {
             const uint32_t x = s & ~DT_LEAF;
-            p = t.lparent[x];
-            const int pd = p == DT_NONE ? -1 : (int)t.ndepth[p];
-            for (uint32_t w = lane; w < 68; w += 32) bufw[w] = 0;
-            __syncwarp();
-            uint32_t len = 0;
-            if (lane == 0) {
-                uint32_t k[8];
-                load32_nc(t.lkey + 32 * (uint64_t)x, k);
-                LinBuf lb{buf, 0};
-                if (t.account)
-                    len = encode_leaf<LinBuf, true>(lb, k, pd, t.lval + 72 * (uint64_t)x,
-                                                    t.lsroot ? t.lsroot + 32 * (uint64_t)x : nullptr, t.err);
-                else
-                    len = encode_leaf<LinBuf, false>(lb, k, pd, t.lval + 32 * (uint64_t)x, nullptr, t.err);
-            }
-            len = __shfl_sync(0xffffffffu, len, 0);
-            uint32_t lmeta;
-            if (len >= 32 || pd < 0) {  // account leaves are >= 70 bytes; a short storage leaf is hashed only as a whole trie
-                if (lane == 0) {
-                    buf[len] |= 0x01;
-                    buf[(len / 136 + 1) * 136 - 1] |= 0x80;
-                }
-                __syncwarp();
-                uint64_t a = kw.hash(buf, len / 136 + 1, lane);
-#pragma unroll
-                for (int q = 0; q < 4; q++) {
-                    uint64_t w = shfl64(a, q);
-                    out[2 * q] = (uint32_t)w;
-                    out[2 * q + 1] = (uint32_t)(w >> 32);
-                }
-                hashed += lane == 0;
-                lmeta = 0;
-            } else {
-                __syncwarp();
-#pragma unroll
-                for (int q = 0; q < 8; q++) out[q] = bufw[q];
-                lmeta = len;
-            }
+            const uint32_t lp = t.lparent[x];
+            const uint32_t lmeta = warp_leaf_ref(t.account, buf, t.lkey + 32 * (uint64_t)x, lp == DT_NONE ? -1 : (int)t.ndepth[lp],
+                                                 t.lval + (uint64_t)t.val_stride * x, t.lsroot ? t.lsroot + 32 * (uint64_t)x : nullptr,
+                                                 t.err, kw, lane, hashed, out);
             if (lane == 0) {
                 store32(t.lref + 32 * (uint64_t)x, out);
                 t.lmeta[x] = (uint8_t)lmeta;
             }
             __syncwarp();
+            p = t.lparent[x];  // (read again, not kept live across the leaf encode: that cost the kernel a spill)
         } else {
             dt_warp_build_node(t, s, buf, kw, lane, hashed, exts, out);
             p = t.nparent[s];
         }
-        bool top = true;
-        for (int hops = 0; p != DT_NONE; hops++) {
-            if (hops > DT_MAX_HOPS) {  // uniform across the warp
-                if (lane == 0) atomicExch(t.err, B200_DEVERR_CORRUPT);
-                top = false;
-                break;
-            }
-            uint32_t last = 0;
-            if (lane == 0) {
-                __threadfence();
-                last = atomicSub(&t.npending[p], 1u) == 1u;
-                __threadfence();
-            }
-            last = __shfl_sync(0xffffffffu, last, 0);
-            if (!last) {
-                top = false;
-                break;
-            }
-            dt_warp_build_node(t, p, buf, kw, lane, hashed, exts, out);
-            p = t.nparent[p];
-        }
-        if (top && lane == 0) store32(t.top_out + (uint64_t)t.top_stride * dt_trie_of(t, s), out);  // the trie's new root
+        if (dt_warp_climb(t, p, buf, kw, lane, hashed, exts, out) && lane == 0)
+            store32(t.top_out + (uint64_t)t.top_stride * dt_trie_of(t, s), out);  // the trie's new root
     }
-    if (lane == 0) {
-        if (hashed) atomicAdd(&t.counters[CNT_HASHED], (unsigned long long)hashed);
-        if (exts) atomicAdd(&t.counters[CNT_EXT], (unsigned long long)exts);
-    }
+    flush_warp_counters(t.counters, hashed, exts);
 }
 
 // ------------------------------------------------------------------------------------------------ two-stage re-hash
@@ -883,61 +892,14 @@ template <int BLOCK>
 __device__ __forceinline__ void dt_thread_build_node(Strip<BLOCK> &s, uint32_t *smem, const DTrieDev &t, uint32_t v,
                                                      uint32_t &hashed, uint32_t &exts, uint32_t (&ref)[8]) {
     s.init(smem);
-    const uint32_t *ch = t.nchild + 16 * (uint64_t)v;
     const int d = t.ndepth[v];
-    uint32_t payload = 1, state_mask = 0, tree_mask = 0, hash_mask = 0;
-    for (int k = 0; k < 16; k++) {
-        uint32_t cw = ch[k];
-        if (cw == DT_NONE) {
-            payload += 1;
-            continue;
-        }
-        bool leaf = (cw & DT_LEAF) != 0;
-        uint32_t id = cw & ~DT_LEAF;
-        uint32_t m = __ldcg(leaf ? t.lmeta + id : t.nmeta + id);
-        payload += (m & META_LEN) ? (m & META_LEN) : 33u;
-        state_mask |= 1u << k;
-        if (!leaf) {
-            if (!(m & META_EXT)) {
-                hash_mask |= 1u << k;
-                if (m & META_LEN) atomicExch(t.err, B200_DEVERR_INLINE_HASH_CHILD);
-            }
-            if (m & META_STORED) tree_mask |= 1u << k;
-        }
-    }
-    put_list_header(s, payload);
-    for (int k = 0; k < 16; k++) {
-        uint32_t cw = ch[k];
-        if (cw == DT_NONE) {
-            s.byte(0x80);
-            continue;
-        }
-        bool leaf = (cw & DT_LEAF) != 0;
-        uint32_t id = cw & ~DT_LEAF;
-        uint32_t m = __ldcg(leaf ? t.lmeta + id : t.nmeta + id);
-        const uint4 *q = reinterpret_cast<const uint4 *>((leaf ? t.lref : t.nref) + 32 * (uint64_t)id);
-        uint4 x = __ldcg(q), y = __ldcg(q + 1);
-        uint32_t cr[8] = {x.x, x.y, x.z, x.w, y.x, y.y, y.z, y.w};
-        uint32_t il = m & META_LEN;
-        if (il == 0) {
-            s.byte(0xa0);
-            s.words8(cr);
-        } else {
-            for (uint32_t b = 0; b < il; b++) s.byte(byte_at(cr, b));
-        }
-    }
-    s.byte(0x80);
-    const uint32_t len = list_header_len(payload) + payload;
+    uint32_t state_mask, tree_mask, hash_mask;
+    const uint32_t payload = dt_branch_payload<true>(t, v, state_mask, tree_mask, hash_mask);
+    dt_put_branch<true>(s, t, v, payload);
     const uint32_t par = t.nparent[v];
     const int pd = par == DT_NONE ? -1 : (int)t.ndepth[par];
-    const bool is_root = pd < 0, need_ext = pd + 1 < d;
-    uint32_t meta = strip_to_ref(s, len, is_root && !need_ext, ref, hashed);
-    if (need_ext) {
-        s.reset();
-        uint32_t elen = encode_extension(s, t.nkey + 32 * (uint64_t)v, (uint32_t)(pd + 1), (uint32_t)d, ref, meta);
-        meta = strip_to_ref(s, elen, is_root, ref, hashed) | META_EXT;
-        exts++;
-    }
+    uint32_t meta = strip_to_ref(s, list_header_len(payload) + payload, pd < 0 && pd + 1 >= d, ref, hashed);
+    meta = thread_finish_node(s, ref, meta, pd, d, t.nkey + 32 * (uint64_t)v, hashed, exts);
     if ((tree_mask | hash_mask) != 0) meta |= META_STORED;
     if ((t.nmeta[v] & META_STORED) && !(meta & META_STORED)) dt_record_removed(t, v);
     store32(t.nref + 32 * (uint64_t)v, ref);
@@ -1001,14 +963,7 @@ __global__ void __launch_bounds__(BLOCK) dt_wavefront_thread_kernel(DTrieDev t, 
         }
         if (top) store32(t.top_out + (uint64_t)t.top_stride * dt_trie_of(t, sd), ref);
     }
-    for (int o = 16; o; o >>= 1) {
-        hashed += __shfl_xor_sync(0xffffffffu, hashed, o);
-        exts += __shfl_xor_sync(0xffffffffu, exts, o);
-    }
-    if ((threadIdx.x & 31) == 0) {
-        if (hashed) atomicAdd(&t.counters[CNT_HASHED], (unsigned long long)hashed);
-        if (exts) atomicAdd(&t.counters[CNT_EXT], (unsigned long long)exts);
-    }
+    flush_counters(t.counters, hashed, exts);
 }
 
 // Stage B: every list entry is one arrival at node p (a dirty child that stage A finished).
@@ -1024,36 +979,12 @@ __global__ void __launch_bounds__(WARPS * 32) dt_climb_kernel(DTrieDev t, const 
     uint32_t hashed = 0, exts = 0;
     const uint32_t count = *count_p;
     for (uint32_t e = blockIdx.x * WARPS + warp; e < count; e += gridDim.x * WARPS) {
-        uint32_t p = arrivals[e];
-        const uint32_t first = p;
+        const uint32_t p = arrivals[e];
         uint32_t out[8];
-        bool top = true;
-        for (int hops = 0; p != DT_NONE; hops++) {
-            if (hops > DT_MAX_HOPS) {
-                if (lane == 0) atomicExch(t.err, B200_DEVERR_CORRUPT);
-                top = false;
-                break;
-            }
-            uint32_t last = 0;
-            if (lane == 0) {
-                __threadfence();
-                last = atomicSub(&t.npending[p], 1u) == 1u;
-                __threadfence();
-            }
-            last = __shfl_sync(0xffffffffu, last, 0);
-            if (!last) {
-                top = false;
-                break;
-            }
-            dt_warp_build_node(t, p, buf, kw, lane, hashed, exts, out);
-            p = t.nparent[p];
-        }
-        if (top && lane == 0) store32(t.top_out + (uint64_t)t.top_stride * dt_trie_of(t, first), out);
+        if (dt_warp_climb(t, p, buf, kw, lane, hashed, exts, out) && lane == 0)
+            store32(t.top_out + (uint64_t)t.top_stride * dt_trie_of(t, p), out);
     }
-    if (lane == 0) {
-        if (hashed) atomicAdd(&t.counters[CNT_HASHED], (unsigned long long)hashed);
-        if (exts) atomicAdd(&t.counters[CNT_EXT], (unsigned long long)exts);
-    }
+    flush_warp_counters(t.counters, hashed, exts);
 }
 
 // ------------------------------------------------------------------------------------------------ TrieUpdates

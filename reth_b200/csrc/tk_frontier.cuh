@@ -16,13 +16,13 @@ __global__ void frontier_kernel(ForestDev f, const uint64_t *__restrict__ bucket
     Strip<BLOCK> s;
     s.init(smem);
     if (b >= 16 || *(volatile int *)f.err != B200_DEVERR_NONE) return;
-    FrontierEntryDev e;
+    FrontierEntryDev &e = out[b];
     for (int i = 0; i < 33; i++) e.as_child[i] = e.as_root[i] = 0;
     e.as_child_len = e.as_root_len = 0;
     uint64_t lo = bucket_offsets[b], hi = bucket_offsets[b + 1];
     if (lo < hi) {
         uint32_t item = f.S[lo];
-        uint32_t ref[8], hashed = 0, meta;
+        uint32_t ref[8], hashed = 0, exts = 0, meta;
         const uint8_t *rootp =
             item < f.n ? f.leaf_ref + 32 * (uint64_t)item : f.node_ref + 32 * (uint64_t)(item - (uint32_t)f.n);
         load32_nc(rootp, ref);
@@ -40,25 +40,14 @@ __global__ void frontier_kernel(ForestDev f, const uint64_t *__restrict__ bucket
             uint32_t d = f.node_masks[v].w;
             uint32_t j0 = f.node_start[v], k = f.node_start[v + 1] - j0;
             uint32_t sm, tm, hm, l, r;
-            uint32_t len = encode_branch(s, f, j0, k, sm, tm, hm, l, r);
+            uint32_t len = encode_branch_u<BLOCK, 16>(s, f, j0, k, sm, tm, hm, l, r);
             meta = strip_to_ref(s, len, false, ref, hashed);
-            if (d > 1) {
-                s.reset();
-                uint32_t elen = encode_extension(s, f.keys + 32 * (uint64_t)l, 1, d, ref, meta);
-                meta = strip_to_ref(s, elen, false, ref, hashed);
-            }
+            meta = thread_finish_node(s, ref, meta, 0, (int)d, f.keys + 32 * (uint64_t)l, hashed, exts);
         }
-        uint32_t il = meta & META_LEN;
-        if (il == 0) {
-            e.as_child_len = 33;
-            e.as_child[0] = 0xa0;
-            for (int i = 0; i < 32; i++) e.as_child[1 + i] = (uint8_t)(ref[i >> 2] >> (8 * (i & 3)));
-        } else {
-            e.as_child_len = (uint8_t)il;
-            for (uint32_t i = 0; i < il; i++) e.as_child[i] = (uint8_t)(ref[i >> 2] >> (8 * (i & 3)));
-        }
+        LinBuf lb{e.as_child, 0};
+        put_child(lb, ref, meta & META_LEN);
+        e.as_child_len = (uint8_t)lb.n;
     }
-    out[b] = e;
 }
 
 // Root from the gathered 16-entry frontier (single thread).

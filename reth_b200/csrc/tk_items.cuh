@@ -20,8 +20,7 @@ __global__ void __launch_bounds__(BLOCK) item_leaf_kernel(ForestDev f, ItemLeave
     const uint64_t step = (uint64_t)gridDim.x * BLOCK;
     for (uint64_t i = (uint64_t)blockIdx.x * BLOCK + threadIdx.x; i < f.n; i += step) {
         s.init(smem);
-        const int pdl = depth_of(f.Lp[i]), pdr = depth_of(f.Lp[i + 1]);
-        const int pd = pdl > pdr ? pdl : pdr;
+        const int pd = parent_depth(f, i, i);
         const uint32_t L = it.key_nibs[i];
         uint32_t ref[8], meta;
         if (L >= 64) {
@@ -42,27 +41,16 @@ __global__ void __launch_bounds__(BLOCK) item_leaf_kernel(ForestDev f, ItemLeave
                     ref[2 * w + 1] = t.y;
                 }
             }
-            meta = META_ISNODE | ((it.flags[i] & 1) ? META_STORED : 0u);
-            if (pd + 1 < (int)L) {  // more than one nibble below its parent (or alone in its trie): extension node
-                uint32_t elen = encode_extension(s, f.keys + 32 * i, (uint32_t)(pd + 1), L, ref, 0u);
-                strip_to_ref(s, elen, pd < 0, ref, hashed);  // >= 35 bytes: always hashed
-                meta |= META_EXT;
-                exts++;
-            }
+            // an extension node when more than one nibble below its parent (or alone in its trie): >= 35 bytes, hashed
+            meta = META_ISNODE | ((it.flags[i] & 1) ? META_STORED : 0u) |
+                   thread_finish_node(s, ref, 0u, pd, (int)L, f.keys + 32 * i, hashed, exts);
         }
         store32(f.leaf_ref + 32 * i, ref);
         f.leaf_meta[i] = (uint8_t)meta;
         f.S[i] = (uint32_t)i;
         f.E[i] = (uint32_t)i;
     }
-    for (int o = 16; o; o >>= 1) {
-        hashed += __shfl_xor_sync(0xffffffffu, hashed, o);
-        exts += __shfl_xor_sync(0xffffffffu, exts, o);
-    }
-    if ((threadIdx.x & 31) == 0) {
-        if (hashed) atomicAdd(&f.counters[CNT_HASHED], (unsigned long long)hashed);
-        if (exts) atomicAdd(&f.counters[CNT_EXT], (unsigned long long)exts);
-    }
+    flush_counters(f.counters, hashed, exts);
 }
 
 cudaError_t launch_item_leaves(const ForestDev &f, const ItemLeavesDev &it, const uint8_t *values, const uint8_t *storage_roots,

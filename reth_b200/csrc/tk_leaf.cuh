@@ -234,8 +234,7 @@ __global__ void __launch_bounds__(BLOCK) leaf_kernel(ForestDev f, const uint8_t 
         s.init(smem);
         uint32_t k[8];
         load32(f.keys + 32 * i, k);
-        int pdl = depth_of(f.Lp[i]), pdr = depth_of(f.Lp[i + 1]);
-        int pd = pdl > pdr ? pdl : pdr;
+        const int pd = parent_depth(f, i, i);
         const uint8_t *vp = ACCOUNT ? values + (uint64_t)sizeof(b200_account_dev) * i : values + 32 * i;
         const uint8_t *sp = (ACCOUNT && storage_roots) ? storage_roots + 32 * i : nullptr;
         uint32_t len = encode_leaf<Strip<BLOCK>, ACCOUNT>(s, k, pd, vp, sp, f.err);
@@ -267,8 +266,7 @@ __global__ void __launch_bounds__(BLOCK) leaf_storage_kernel(ForestDev f, const 
         uint32_t k[8], v[8], ref[8];
         load32(f.keys + 32 * i, k);
         load32(values + 32 * i, v);
-        const int pdl = depth_of(f.Lp[i]), pdr = depth_of(f.Lp[i + 1]);
-        const int pd = pdl > pdr ? pdl : pdr;
+        const int pd = parent_depth(f, i, i);
         uint32_t meta;
         if (pd >= 0 && pd <= 26) {
             uint32_t zi = 8, zword = 0;

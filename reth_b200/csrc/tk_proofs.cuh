@@ -8,12 +8,6 @@
 // the trie (crates/trie/trie/src/proof/mod.rs).  An extension node and the branch below it are two proof nodes; the walk
 // stops at a leaf (inclusion, or exclusion by a different key), at an empty slot, or inside an extension whose nibbles
 // differ from the key.  One thread per target; two passes (sizes, then bytes) around an exclusive scan.
-struct CountBuf {  // sizing pass: same interface as LinBuf, nothing is written
-    uint32_t n;
-    __device__ __forceinline__ void byte(uint32_t) { n++; }
-    __device__ __forceinline__ void tail32(const uint32_t (&)[8], uint32_t b0) { n += 32 - b0; }
-    __device__ __forceinline__ void words8(const uint32_t (&)[8]) { n += 32; }
-};
 
 // keccak256 of `len` bytes at an arbitrarily aligned global address (thread-serial; proofs are not a throughput path)
 static __device__ void dt_keccak_global(const uint8_t *p, uint32_t len, uint32_t (&dig)[8]) {
@@ -45,43 +39,6 @@ static __device__ void dt_keccak_global(const uint8_t *p, uint32_t len, uint32_t
         dig[2 * i] = (uint32_t)a[i];
         dig[2 * i + 1] = (uint32_t)(a[i] >> 32);
     }
-}
-
-static __device__ __forceinline__ uint32_t dt_branch_rlp_len(const DTrieDev &t, uint32_t v, uint32_t &payload) {
-    payload = 1;
-    for (int s = 0; s < 16; s++) {
-        uint32_t cw = t.nchild[16 * (uint64_t)v + s];
-        if (cw == DT_NONE) {
-            payload += 1;
-        } else {
-            uint32_t m = (cw & DT_LEAF) ? t.lmeta[cw & ~DT_LEAF] : t.nmeta[cw];
-            payload += (m & META_LEN) ? (m & META_LEN) : 33u;
-        }
-    }
-    return list_header_len(payload) + payload;
-}
-static __device__ void dt_write_branch_rlp(const DTrieDev &t, uint32_t v, uint32_t payload, uint8_t *dst) {
-    LinBuf lb{dst, 0};
-    put_list_header(lb, payload);
-    for (int s = 0; s < 16; s++) {
-        uint32_t cw = t.nchild[16 * (uint64_t)v + s];
-        if (cw == DT_NONE) {
-            lb.byte(0x80);
-            continue;
-        }
-        bool leaf = (cw & DT_LEAF) != 0;
-        uint32_t id = cw & ~DT_LEAF, m = leaf ? t.lmeta[id] : t.nmeta[id];
-        uint32_t ref[8];
-        load32_nc((leaf ? t.lref : t.nref) + 32 * (uint64_t)id, ref);
-        uint32_t il = m & META_LEN;
-        if (il == 0) {
-            lb.byte(0xa0);
-            lb.words8(ref);
-        } else {
-            for (uint32_t b = 0; b < il; b++) lb.byte(byte_at(ref, b));
-        }
-    }
-    lb.byte(0x80);
 }
 
 // Walks target `key` in trie `trie`.  WRITE = false: returns node / byte counts.  WRITE = true: writes the nodes at
@@ -130,8 +87,9 @@ static __device__ void dt_proof_walk(const DTrieDev &t, uint32_t trie, const uin
         const uint32_t v = cur;
         const int d = t.ndepth[v];
         const uint8_t *nk = t.nkey + 32 * (uint64_t)v;
-        uint32_t payload;
-        const uint32_t blen = dt_branch_rlp_len(t, v, payload);
+        uint32_t sm, tm, hm;
+        const uint32_t payload = dt_branch_payload<false>(t, v, sm, tm, hm);
+        const uint32_t blen = list_header_len(payload) + payload;
         const ushort4 mk = t.nmasks[v];
         const uint32_t masks = ((uint32_t)mk.z << 16) | mk.y;
         const bool ext = pd + 1 < d;
@@ -147,7 +105,8 @@ static __device__ void dt_proof_walk(const DTrieDev &t, uint32_t trie, const uin
                 uint8_t *ext_at = rlp + byte_base + n_bytes;
                 uint8_t tmp[544];
                 uint8_t *br_at = matches ? ext_at + elen : tmp;
-                dt_write_branch_rlp(t, v, payload, br_at);
+                LinBuf br{br_at, 0};
+                dt_put_branch<false>(br, t, v, payload);
                 uint32_t child[8] = {0, 0, 0, 0, 0, 0, 0, 0};
                 if (blen >= 32) dt_keccak_global(br_at, blen, child);
                 else
@@ -159,7 +118,10 @@ static __device__ void dt_proof_walk(const DTrieDev &t, uint32_t trie, const uin
             if (!matches) return;
             begin_node(blen, d, masks);
         } else {
-            if (WRITE) dt_write_branch_rlp(t, v, payload, rlp + byte_base + n_bytes);
+            if (WRITE) {
+                LinBuf br{rlp + byte_base + n_bytes, 0};
+                dt_put_branch<false>(br, t, v, payload);
+            }
             begin_node(blen, d, masks);
         }
         pd = d;

@@ -53,17 +53,6 @@ struct Strip {
             }
         }
     }
-    // bytes [0, len) of a 32-byte string held as 8 little-endian words (an inline child reference, len < 32): whole
-    // words, then the 0..3 bytes of the partial one.  Every word index is a constant, so the string stays in registers.
-    __device__ __forceinline__ void head32(const uint32_t (&x)[8], uint32_t len) {
-        uint32_t part = 0;
-#pragma unroll
-        for (int i = 0; i < 8; i++) {
-            if (4u * i + 4 <= len) word(x[i]);
-            else if (4u * i < len) part = x[i];
-        }
-        for (uint32_t b = 0; b < (len & 3); b++) byte((part >> (8 * b)) & 0xff);
-    }
     __device__ __forceinline__ uint32_t length() const { return nw * 4 + nb; }
     __device__ __forceinline__ uint32_t read_word(uint32_t i) const { return w[i * BLOCK]; }
     // Keccak pad10*1 to a multiple of the 136-byte rate; returns the number of rate blocks.
@@ -124,6 +113,13 @@ static __device__ __forceinline__ void load32_nc(const uint8_t *p, uint32_t (&x)
     x[0] = a.x; x[1] = a.y; x[2] = a.z; x[3] = a.w;
     x[4] = b.x; x[5] = b.y; x[6] = b.z; x[7] = b.w;
 }
+static __device__ __forceinline__ void load32_cg(const uint8_t *p, uint32_t (&x)[8]) {
+    // L1-bypassing loads: data written by other SMs earlier in the same kernel (the wavefronts)
+    const uint4 *q = reinterpret_cast<const uint4 *>(p);
+    uint4 a = __ldcg(q), b = __ldcg(q + 1);
+    x[0] = a.x; x[1] = a.y; x[2] = a.z; x[3] = a.w;
+    x[4] = b.x; x[5] = b.y; x[6] = b.z; x[7] = b.w;
+}
 static __device__ __forceinline__ void store32(uint8_t *p, const uint32_t (&x)[8]) {
     uint4 *q = reinterpret_cast<uint4 *>(p);
     q[0] = make_uint4(x[0], x[1], x[2], x[3]);
@@ -135,6 +131,27 @@ static __device__ __forceinline__ uint32_t key_nibble_mem(const uint8_t *key, ui
     return (i & 1) ? (b & 15) : (b >> 4);
 }
 static __device__ __forceinline__ int depth_of(uint8_t lp) { return lp == 0xFF ? -1 : (int)lp; }
+// depth of the parent of the item spanning leaves [l, r]: the deeper of its two boundary gaps (-1: the item is a whole trie)
+static __device__ __forceinline__ int parent_depth(const ForestDev &f, uint64_t l, uint64_t r) {
+    const int pdl = depth_of(f.Lp[l]), pdr = depth_of(f.Lp[r + 1]);
+    return pdl > pdr ? pdl : pdr;
+}
+
+// Node / extension counts of a build (CNT_HASHED, CNT_EXT).  Warp-per-item kernels: lane 0 holds the warp's counts.
+static __device__ __forceinline__ void flush_warp_counters(unsigned long long *counters, uint32_t hashed, uint32_t exts) {
+    if ((threadIdx.x & 31) == 0) {
+        if (hashed) atomicAdd(&counters[CNT_HASHED], (unsigned long long)hashed);
+        if (exts) atomicAdd(&counters[CNT_EXT], (unsigned long long)exts);
+    }
+}
+// thread-per-item kernels: one atomic per warp and counter
+static __device__ __forceinline__ void flush_counters(unsigned long long *counters, uint32_t hashed, uint32_t exts) {
+    for (int o = 16; o; o >>= 1) {
+        hashed += __shfl_xor_sync(0xffffffffu, hashed, o);
+        exts += __shfl_xor_sync(0xffffffffu, exts, o);
+    }
+    flush_warp_counters(counters, hashed, exts);
+}
 
 // number of leading zero BYTES of a 32-byte big-endian integer held as LE words (32 if zero)
 static __device__ __forceinline__ uint32_t leading_zero_bytes(const uint32_t (&x)[8]) {
@@ -152,6 +169,33 @@ static __device__ __forceinline__ uint32_t byte_at(const uint32_t (&x)[8], uint3
     return (w >> (8 * (j & 3))) & 0xff;
 }
 
+// byte writer over a linear buffer (a warp's shared buffer written by one lane, a proof node in global memory)
+struct LinBuf {
+    uint8_t *p;
+    uint32_t n;
+    __device__ __forceinline__ void byte(uint32_t b) { p[n++] = (uint8_t)b; }
+    __device__ __forceinline__ void word(uint32_t x) {
+        p[n++] = (uint8_t)x;
+        p[n++] = (uint8_t)(x >> 8);
+        p[n++] = (uint8_t)(x >> 16);
+        p[n++] = (uint8_t)(x >> 24);
+    }
+    __device__ __forceinline__ void words8(const uint32_t (&x)[8]) {
+#pragma unroll
+        for (int i = 0; i < 8; i++) word(x[i]);
+    }
+    __device__ __forceinline__ void tail32(const uint32_t (&x)[8], uint32_t b0) {
+        for (uint32_t b = b0; b < 32; b++) byte(byte_at(x, b));
+    }
+};
+struct CountBuf {  // sizing pass: same interface as LinBuf, nothing is written
+    uint32_t n;
+    __device__ __forceinline__ void byte(uint32_t) { n++; }
+    __device__ __forceinline__ void word(uint32_t) { n += 4; }
+    __device__ __forceinline__ void words8(const uint32_t (&)[8]) { n += 32; }
+    __device__ __forceinline__ void tail32(const uint32_t (&)[8], uint32_t b0) { n += 32 - b0; }
+};
+
 // RLP list header for a payload < 65536 bytes
 template <class W>
 static __device__ __forceinline__ void put_list_header(W &s, uint32_t payload) {
@@ -168,4 +212,25 @@ static __device__ __forceinline__ void put_list_header(W &s, uint32_t payload) {
 }
 static __device__ __forceinline__ uint32_t list_header_len(uint32_t payload) {
     return payload < 56 ? 1 : (payload < 256 ? 2 : 3);
+}
+
+// A child's RlpNode inside its parent: 0xa0 + the 32-byte hash (inline_len == 0), or the child's own RLP of inline_len
+// < 32 bytes, written as whole words and then the 0..3 bytes of the partial one.  Every word index is a constant, so
+// the reference stays in registers (a run-time byte index would put it in local memory).
+template <class W>
+static __device__ __forceinline__ void put_child(W &s, const uint32_t (&ref)[8], uint32_t inline_len) {
+    if (inline_len == 0) {
+        s.byte(0xa0);
+        s.words8(ref);
+        return;
+    }
+    uint32_t part = 0;
+#pragma unroll
+    for (int i = 0; i < 8; i++) {
+        if (4u * i + 4 <= inline_len) s.word(ref[i]);
+        part |= (4u * i < inline_len && inline_len < 4u * i + 4) ? ref[i] : 0u;
+    }
+#pragma unroll
+    for (uint32_t b = 0; b < 3; b++)
+        if (b < (inline_len & 3)) s.byte((part >> (8 * b)) & 0xff);
 }

@@ -50,58 +50,25 @@ struct WarpKeccak {
             if (lane0) a ^= KECCAK_RC[r];
         }
     }
-    // keccak256 of buf[0 .. blocks*136) (already padded); digest word i ends up in lane i (i < 4)
-    __device__ __forceinline__ uint64_t hash(const uint8_t *buf, uint32_t blocks, int lane) const {
+    // keccak256 of buf[0 .. blocks*136) (already padded) -> 8 little-endian digest words in every lane
+    __device__ __forceinline__ void digest(const uint8_t *buf, uint32_t blocks, int lane, uint32_t (&out)[8]) const {
         uint64_t a = 0;
         const uint64_t *w = reinterpret_cast<const uint64_t *>(buf);
         for (uint32_t b = 0; b < blocks; b++) {
             if (lane < 17) a ^= w[17 * b + lane];
             permute(a);
         }
-        return a;
-    }
-};
-
-// byte writer over a warp's linear shared buffer (single-lane use)
-struct LinBuf {
-    uint8_t *p;
-    uint32_t n;
-    __device__ __forceinline__ void byte(uint32_t b) { p[n++] = (uint8_t)b; }
-    __device__ __forceinline__ void tail32(const uint32_t (&x)[8], uint32_t b0) {
-        for (uint32_t b = b0; b < 32; b++) byte(byte_at(x, b));
-    }
-    __device__ __forceinline__ void words8(const uint32_t (&x)[8]) {
 #pragma unroll
-        for (int i = 0; i < 8; i++) {
-            p[n++] = (uint8_t)x[i];
-            p[n++] = (uint8_t)(x[i] >> 8);
-            p[n++] = (uint8_t)(x[i] >> 16);
-            p[n++] = (uint8_t)(x[i] >> 24);
+        for (int i = 0; i < 4; i++) {  // digest word i is in lane i
+            uint64_t x = shfl64(a, i);
+            out[2 * i] = (uint32_t)x;
+            out[2 * i + 1] = (uint32_t)(x >> 32);
         }
     }
 };
 
 constexpr int WARP_BUF = 560;  // 4 rate blocks + slack, 16-byte multiple
 
-// fetch_child with loads that bypass L1 (data produced by other SMs earlier in the SAME kernel: the wavefront)
-template <bool COHERENT>
-__device__ __forceinline__ ChildInfo fetch_child_c(const ForestDev &f, uint32_t j0, uint32_t c) {
-    if (!COHERENT) return fetch_child(f, j0, c);
-    ChildInfo ci;
-    if (c == 0) {
-        uint32_t g = f.gap_sorted[j0];
-        ci.id = f.E[g - 1];
-        ci.nib = f.nibs[g] >> 4;
-    } else {
-        uint32_t g = f.gap_sorted[j0 + c - 1];
-        ci.id = f.S[g];
-        ci.nib = f.nibs[g] & 15;
-    }
-    ci.meta = ci.id < f.n ? __ldcg(f.leaf_meta + ci.id) : __ldcg(f.node_meta + (ci.id - (uint32_t)f.n));
-    return ci;
-}
-
-// (Same steps as the tail of warp_build_node below, which keeps its own copy so that its SASS stays as measured.)
 // The assembled branch RLP (`total` bytes, padded into `blocks` rate blocks of `buf`) -> RlpNode of the node as seen from a
 // parent at depth pd: hashed if >= 32 bytes (or a trie root), wrapped in an extension node when more than one nibble
 // separates it from the parent.  Uniform control flow: all 32 lanes call.  Returns the meta byte (inline length | META_EXT).
@@ -112,13 +79,7 @@ __device__ __forceinline__ uint32_t warp_finish_node(uint8_t *buf, uint32_t tota
     bool is_root = pd < 0, need_ext = pd + 1 < d;
     uint32_t meta;
     if (total >= 32 || (is_root && !need_ext)) {
-        uint64_t a = kw.hash(buf, blocks, lane);
-#pragma unroll
-        for (int i = 0; i < 4; i++) {
-            uint64_t w = shfl64(a, i);
-            out[2 * i] = (uint32_t)w;
-            out[2 * i + 1] = (uint32_t)(w >> 32);
-        }
+        kw.digest(buf, blocks, lane, out);
         meta = 0;
         hashed += lane == 0;
     } else {
@@ -140,13 +101,7 @@ __device__ __forceinline__ uint32_t warp_finish_node(uint8_t *buf, uint32_t tota
         elen = __shfl_sync(0xffffffffu, elen, 0);
         __syncwarp();
         if (elen >= 32 || is_root) {
-            uint64_t a = kw.hash(buf, 1, lane);
-#pragma unroll
-            for (int i = 0; i < 4; i++) {
-                uint64_t w = shfl64(a, i);
-                out[2 * i] = (uint32_t)w;
-                out[2 * i + 1] = (uint32_t)(w >> 32);
-            }
+            kw.digest(buf, 1, lane, out);
             meta = META_EXT;
             hashed += lane == 0;
         } else {
@@ -157,6 +112,39 @@ __device__ __forceinline__ uint32_t warp_finish_node(uint8_t *buf, uint32_t tota
         exts += lane == 0;
     }
     return meta;
+}
+
+// One warp re-encodes a leaf with parent depth pd (lane 0 writes the RLP) -> its RlpNode in `out`: hashed when >= 32 bytes
+// or a whole trie, else the RLP itself.  Account leaves are >= 70 bytes: always hashed.  All 32 lanes call; returns the
+// meta byte (inline length, 0 = hashed).
+__device__ __forceinline__ uint32_t warp_leaf_ref(bool account, uint8_t *buf, const uint8_t *key, int pd, const uint8_t *val,
+                                                  const uint8_t *sroot, int *err, const WarpKeccak &kw, int lane, uint32_t &hashed,
+                                                  uint32_t (&out)[8]) {
+    uint32_t *bufw = reinterpret_cast<uint32_t *>(buf);
+    for (uint32_t w = lane; w < 68; w += 32) bufw[w] = 0;
+    __syncwarp();
+    uint32_t len = 0;
+    if (lane == 0) {
+        uint32_t k[8];
+        load32_nc(key, k);
+        LinBuf lb{buf, 0};
+        len = account ? encode_leaf<LinBuf, true>(lb, k, pd, val, sroot, err) : encode_leaf<LinBuf, false>(lb, k, pd, val, nullptr, err);
+    }
+    len = __shfl_sync(0xffffffffu, len, 0);
+    if (len >= 32 || pd < 0) {
+        if (lane == 0) {
+            buf[len] |= 0x01;
+            buf[(len / 136 + 1) * 136 - 1] |= 0x80;
+        }
+        __syncwarp();
+        kw.digest(buf, len / 136 + 1, lane, out);
+        hashed += lane == 0;
+        return 0;
+    }
+    __syncwarp();
+#pragma unroll
+    for (int q = 0; q < 8; q++) out[q] = bufw[q];
+    return len;
 }
 
 // One warp builds branch node v of depth d (all 32 lanes must call).  Returns through lane 0's stores.
@@ -173,16 +161,10 @@ __device__ __forceinline__ void warp_build_node(const ForestDev &f, uint32_t v, 
     uint32_t ref[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     uint32_t lext = 0, rext = 0;
     if (has) {
-        ci = fetch_child_c<COHERENT>(f, j0, (uint32_t)lane);
+        ci = fetch_child<COHERENT>(f, j0, (uint32_t)lane);
         const uint8_t *rp = ci.id < n ? f.leaf_ref + 32 * (uint64_t)ci.id : f.node_ref + 32 * (uint64_t)(ci.id - n);
-        if (COHERENT) {
-            const uint4 *q = reinterpret_cast<const uint4 *>(rp);
-            uint4 x = __ldcg(q), y = __ldcg(q + 1);
-            ref[0] = x.x; ref[1] = x.y; ref[2] = x.z; ref[3] = x.w;
-            ref[4] = y.x; ref[5] = y.y; ref[6] = y.z; ref[7] = y.w;
-        } else {
-            load32_nc(rp, ref);
-        }
+        if (COHERENT) load32_cg(rp, ref);
+        else load32_nc(rp, ref);
         if (lane == 0) lext = ci.id < n ? ci.id : f.node_l[ci.id - n];
         if ((uint32_t)lane == k) rext = ci.id < n ? ci.id : f.node_r[ci.id - n];
     }
@@ -213,19 +195,8 @@ __device__ __forceinline__ void warp_build_node(const ForestDev &f, uint32_t v, 
         put_list_header(lb, payload);
     }
     if (has) {  // child bytes at hdr + (lengths of earlier children) + (empty slots before this nibble)
-        uint32_t off = hdr + (incl - clen) + (ci.nib - (uint32_t)lane);
-        if ((ci.meta & META_LEN) == 0) {
-            buf[off++] = 0xa0;
-#pragma unroll
-            for (int i = 0; i < 8; i++) {
-                buf[off++] = (uint8_t)ref[i];
-                buf[off++] = (uint8_t)(ref[i] >> 8);
-                buf[off++] = (uint8_t)(ref[i] >> 16);
-                buf[off++] = (uint8_t)(ref[i] >> 24);
-            }
-        } else {
-            for (uint32_t b = 0; b < clen; b++) buf[off++] = (uint8_t)byte_at(ref, b);
-        }
+        LinBuf lb{buf + hdr + (incl - clen) + (ci.nib - (uint32_t)lane), 0};
+        put_child(lb, ref, ci.meta & META_LEN);
     }
     {  // empty slots: lane e < 16 owns nibble e
         uint32_t cb = __popc(state_mask & ((1u << (lane & 15)) - 1));
@@ -238,56 +209,8 @@ __device__ __forceinline__ void warp_build_node(const ForestDev &f, uint32_t v, 
         buf[blocks * 136 - 1] |= 0x80;
     }
     __syncwarp();
-    // ---- parent depth, extension, hash (uniform control flow)
-    int pdl = depth_of(f.Lp[l]), pdr = depth_of(f.Lp[(uint64_t)r + 1]);
-    int pd = pdl > pdr ? pdl : pdr;
-    bool is_root = pd < 0, need_ext = pd + 1 < d;
-    uint32_t meta;
-    if (total >= 32 || (is_root && !need_ext)) {
-        uint64_t a = kw.hash(buf, blocks, lane);
-#pragma unroll
-        for (int i = 0; i < 4; i++) {
-            uint64_t w = shfl64(a, i);
-            out[2 * i] = (uint32_t)w;
-            out[2 * i + 1] = (uint32_t)(w >> 32);
-        }
-        meta = 0;
-        hashed += lane == 0;
-    } else {
-#pragma unroll
-        for (int i = 0; i < 8; i++) out[i] = bufw[i];
-        meta = total;
-    }
-    if (need_ext) {
-        __syncwarp();
-        for (uint32_t w = lane; w < 34; w += 32) bufw[w] = 0;
-        __syncwarp();
-        uint32_t elen = 0;
-        if (lane == 0) {
-            LinBuf lb{buf, 0};
-            elen = encode_extension(lb, f.keys + 32 * (uint64_t)l, (uint32_t)(pd + 1), (uint32_t)d, out, meta);
-            buf[elen] |= 0x01;
-            buf[135] |= 0x80;
-        }
-        elen = __shfl_sync(0xffffffffu, elen, 0);
-        __syncwarp();
-        if (elen >= 32 || is_root) {
-            uint64_t a = kw.hash(buf, 1, lane);
-#pragma unroll
-            for (int i = 0; i < 4; i++) {
-                uint64_t w = shfl64(a, i);
-                out[2 * i] = (uint32_t)w;
-                out[2 * i + 1] = (uint32_t)(w >> 32);
-            }
-            meta = META_EXT;
-            hashed += lane == 0;
-        } else {
-#pragma unroll
-            for (int i = 0; i < 8; i++) out[i] = bufw[i];
-            meta = elen | META_EXT;
-        }
-        exts += lane == 0;
-    }
+    uint32_t meta = warp_finish_node(buf, total, blocks, d, parent_depth(f, l, r), f.keys + 32 * (uint64_t)l, kw, lane, hashed,
+                                     exts, out);
     if (lane == 0) {
         if ((tree_mask | hash_mask) != 0) meta |= META_STORED;
         store32(f.node_ref + 32 * (uint64_t)v, out);
@@ -316,8 +239,5 @@ __global__ void __launch_bounds__(WARPS * 32) branch_warp_kernel(ForestDev f, co
         uint32_t out[8];
         warp_build_node<false>(f, __ldg(node_order + p64), d, sbuf[warp], kw, lane, hashed, exts, out);
     }
-    if (lane == 0) {
-        if (hashed) atomicAdd(&f.counters[CNT_HASHED], (unsigned long long)hashed);
-        if (exts) atomicAdd(&f.counters[CNT_EXT], (unsigned long long)exts);
-    }
+    flush_warp_counters(f.counters, hashed, exts);
 }

@@ -58,7 +58,6 @@ __global__ void __launch_bounds__(WARPS * 32) wavefront_kernel(ForestDev f, uint
     if (*(volatile int *)f.err != B200_DEVERR_NONE) return;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     uint8_t *buf = sbuf[warp];
-    uint32_t *bufw = reinterpret_cast<uint32_t *>(buf);
     WarpKeccak kw;
     kw.init(lane);
     uint32_t hashed = 0, exts = 0;
@@ -66,11 +65,6 @@ __global__ void __launch_bounds__(WARPS * 32) wavefront_kernel(ForestDev f, uint
     if (t >= m) return;
     const uint32_t i = idx[t];
     // ---- the leaf
-    for (uint32_t w = lane; w < 68; w += 32) bufw[w] = 0;
-    __syncwarp();
-    int pdl = depth_of(f.Lp[i]), pdr = depth_of(f.Lp[(uint64_t)i + 1]);
-    int pd = pdl > pdr ? pdl : pdr;
-    uint32_t len = 0;
     if (lane == 0) {
         const uint64_t *src = reinterpret_cast<const uint64_t *>(new_accts + 72 * t);
         uint64_t *dst = reinterpret_cast<uint64_t *>(accts + 72 * (uint64_t)i);
@@ -81,28 +75,10 @@ __global__ void __launch_bounds__(WARPS * 32) wavefront_kernel(ForestDev f, uint
             load32(new_sroots + 32 * t, r);
             store32(sroots + 32 * (uint64_t)i, r);
         }
-        uint32_t k[8];
-        load32(f.keys + 32 * (uint64_t)i, k);
-        LinBuf lb{buf, 0};
-        len = encode_leaf<LinBuf, true>(lb, k, pd, new_accts + 72 * t,
-                                        sroots ? (new_sroots ? new_sroots + 32 * t : sroots + 32 * (uint64_t)i) : nullptr,
-                                        f.err);
-        buf[len] |= 0x01;
-        buf[(len / 136 + 1) * 136 - 1] |= 0x80;
     }
-    len = __shfl_sync(0xffffffffu, len, 0);
-    __syncwarp();
     uint32_t out[8];
-    {
-        uint64_t a = kw.hash(buf, len / 136 + 1, lane);  // account leaves are >= 70 bytes: always hashed
-#pragma unroll
-        for (int q = 0; q < 4; q++) {
-            uint64_t w = shfl64(a, q);
-            out[2 * q] = (uint32_t)w;
-            out[2 * q + 1] = (uint32_t)(w >> 32);
-        }
-        hashed += lane == 0;
-    }
+    warp_leaf_ref(true, buf, f.keys + 32 * (uint64_t)i, parent_depth(f, i, i), new_accts + 72 * t,
+                  sroots ? (new_sroots ? new_sroots + 32 * t : sroots + 32 * (uint64_t)i) : nullptr, f.err, kw, lane, hashed, out);
     if (lane == 0) {
         store32(f.leaf_ref + 32 * (uint64_t)i, out);
         f.leaf_meta[i] = 0;
@@ -111,10 +87,7 @@ __global__ void __launch_bounds__(WARPS * 32) wavefront_kernel(ForestDev f, uint
     // ---- climb
     bool top = warp_climb(f, leaf_parent[i], node_parent, pending, dirty_list, dirty_count, buf, kw, lane, hashed, exts, out);
     if (top && lane == 0) store32(root_out, out);  // this warp re-hashed the root (or the only leaf)
-    if (lane == 0) {
-        if (hashed) atomicAdd(&f.counters[CNT_HASHED], (unsigned long long)hashed);
-        if (exts) atomicAdd(&f.counters[CNT_EXT], (unsigned long long)exts);
-    }
+    flush_warp_counters(f.counters, hashed, exts);
 }
 
 // ---- two-stage variant for large dirty sets -----------------------------------------------------------------------
@@ -150,8 +123,7 @@ __global__ void __launch_bounds__(BLOCK) wavefront_thread_kernel(
         }
         uint32_t k[8];
         load32(f.keys + 32 * (uint64_t)i, k);
-        int pdl = depth_of(f.Lp[i]), pdr = depth_of(f.Lp[(uint64_t)i + 1]);
-        int pd = pdl > pdr ? pdl : pdr;
+        const int pd = parent_depth(f, i, i);
         uint32_t len = encode_leaf<Strip<BLOCK>, true>(
             s, k, pd, new_accts + 72 * t, sroots ? (new_sroots ? new_sroots + 32 * t : sroots + 32 * (uint64_t)i) : nullptr,
             f.err);
@@ -182,14 +154,7 @@ __global__ void __launch_bounds__(BLOCK) wavefront_thread_kernel(
         }
         if (top) store32(root_out, ref);
     }
-    for (int o = 16; o; o >>= 1) {
-        hashed += __shfl_xor_sync(0xffffffffu, hashed, o);
-        exts += __shfl_xor_sync(0xffffffffu, exts, o);
-    }
-    if ((threadIdx.x & 31) == 0) {
-        if (hashed) atomicAdd(&f.counters[CNT_HASHED], (unsigned long long)hashed);
-        if (exts) atomicAdd(&f.counters[CNT_EXT], (unsigned long long)exts);
-    }
+    flush_counters(f.counters, hashed, exts);
 }
 
 template <int WARPS>
@@ -211,8 +176,5 @@ __global__ void __launch_bounds__(WARPS * 32) climb_kernel(ForestDev f, const ui
                               exts, out);
         if (top && lane == 0) store32(root_out, out);
     }
-    if (lane == 0) {
-        if (hashed) atomicAdd(&f.counters[CNT_HASHED], (unsigned long long)hashed);
-        if (exts) atomicAdd(&f.counters[CNT_EXT], (unsigned long long)exts);
-    }
+    flush_warp_counters(f.counters, hashed, exts);
 }

@@ -31,7 +31,7 @@ def test_dynamic_tries_two_stage_rehash_under_cpu_emulation():
     warp-climb re-hash (B200_DT_TWO_STAGE_MIN=0; by default only dirty sets above 4096 entries take it)."""
     r = subprocess.run([sys.executable, "-m", "pytest", "tests/test_gpu_dtrie.py", "tests/test_gpu_dstate.py", "-m", "gpu",
                         "--emu", "-q", "-x", "-p", "no:cacheprovider", "-k",
-                        "random_blocks or shrink or clustered or sharded_state_matches or new_contract or lifecycle"],
+                        "random_blocks or shrink or clustered or sharded_state_matches or new_contract or lifecycle or inline_children"],
                        cwd=ROOT, capture_output=True, text=True, timeout=1500,
                        env=dict(os.environ, B200_DT_TWO_STAGE_MIN="0", B200_DT_FUSED_MAX="0"))
     tail = (r.stdout + r.stderr)[-3000:]

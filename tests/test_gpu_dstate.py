@@ -421,6 +421,65 @@ def test_new_contract_with_many_slots_in_one_block(eng):
     h.ds.close()
 
 
+def clustered_slots(rng, n_clusters):
+    """Slots in clusters of 2..16 keys that differ only in their last nibble.  A cluster is one depth-63 branch whose
+    leaves are inline: 3, 5 or 6 bytes of RLP for a value < 0x80, < 0x100 or < 0x10000.  The branch is 18 - n + (the
+    leaves' lengths) bytes; below 32 it is itself inline, under the extension that leads to it from the shallow branch
+    where the clusters part."""
+    slots = {}
+    for _ in range(n_clusters):
+        key = bytearray(rkey(rng))
+        for nib in rng.choice(16, int(rng.integers(2, 17)), replace=False):
+            key[31] = (key[31] & 0xF0) | int(nib)
+            slots[bytes(key)] = int(rng.integers(1, (0x80, 0x100, 0x10000)[rng.integers(0, 3)]))
+    return slots
+
+
+def test_inline_children_of_clustered_slots(eng):
+    """Storage tries whose branches have inline (< 32 byte) children: the inline-child paths of the warp and thread node
+    builders and of the proof encoder.  Small blocks first, then one block of more than 8192 slot entries (the multi-launch
+    restructure and the two-stage re-hash at the default thresholds); the slot proofs of clustered keys chain to the roots."""
+    from tests.test_gpu_proofs import verify
+    rng = np.random.default_rng(515)
+    st = random_state(rng, 200, with_storage=0.0)
+    owners = sorted(st)[:24]
+    for k in owners:
+        st[k] = (st[k][0], clustered_slots(rng, int(rng.integers(1, 5))))
+    h = Harness(eng, st)
+    for step in range(3):
+        block = {}
+        for i in rng.choice(len(owners), 6, replace=False):
+            k = owners[i]
+            slots = clustered_slots(rng, 2)
+            for s in sorted(h.state[k][1])[:4]:               # changed and deleted members of existing clusters
+                slots[s] = 0 if rng.random() < 0.5 else int(rng.integers(1, 0x10000))
+            block[k] = (EXISTS | UNCHANGED, acct(0), slots)
+        h.commit(block)
+    block, n = {}, 0
+    for k in owners:
+        slots = clustered_slots(rng, 40)
+        n += len(slots)
+        block[k] = (EXISTS | UNCHANGED, acct(0), slots)
+    assert n > 8192
+    h.commit(block)
+    _, keys, _, skeys, svals, offs = flatten(h.state)
+    sroots = oracle.storage_roots(skeys, svals, offs)
+    index = {k: i for i, k in enumerate(sorted(h.state))}
+    inline_lengths = set()
+    for k in owners:
+        have = sorted(h.state[k][1])
+        near = [s[:31] + bytes([s[31] ^ 0x0F]) for s in have[:4]]   # same cluster prefix, maybe absent
+        tgt = have[:12] + near
+        sroot, proofs = h.ds.storage_proofs(k, np.frombuffer(b"".join(tgt), np.uint8).reshape(-1, 32))
+        assert sroot == sroots[index[k]].tobytes()
+        for s, proof in zip(tgt, proofs):
+            v = h.state[k][1].get(s)
+            verify(sroot, s, proof, None if v is None else oracle.encode_u256(v))
+            inline_lengths |= {len(node) for node in proof[1:] if len(node) < 32}
+    assert {n % 4 for n in inline_lengths} == {0, 1, 2, 3}      # every tail length of an inline child reference
+    h.ds.close()
+
+
 def test_merkle_stage_incremental_equals_rebuild(eng):
     """The three stages end to end: a full pass (AccountHashing, StorageHashing, MerkleStage rebuild), then ranges of
     changes through MerkleStage.execute_incremental (incremental hashing + the resident state).  After every range the
