@@ -559,6 +559,37 @@ B200_API int32_t b200_dstate_multiproof(b200_dstate *, const uint8_t *acct_keys3
                                         const uint64_t *slot_seg_offsets, const uint8_t *slot_keys32, b200_proofs *account_proofs,
                                         uint8_t *storage_roots32, b200_proofs *storage_proofs);
 B200_API void b200_proofs_release(b200_proofs *);
+/* Execution witness of one block (reth's TrieWitness::compute, crates/trie/trie/src/witness.rs; what debug_executionWitness
+ * and stateless re-execution consume): { keccak(node) -> node RLP } of every trie node needed to apply the block to this
+ * state, computed on the device from the resident state, which stays unchanged.  The block comes in exactly the layout of
+ * b200_dstate_apply and with its rules: a destroyed entry is removed and its storage counts as wiped, an entry with bit 1 set
+ * for an absent account is ignored (its key and slots are still proved); the slot entries of every entry are targets.
+ * The map holds, keyed by the keccak of its RLP (nodes shorter than 32 bytes included):
+ *   - every node of the proof of every target — the account entries, their slot entries, and every slot a wiped storage
+ *     holds — with both nodes of every extension on a proof path, the branch below a diverging extension included;
+ *   - the nodes a sparse trie has to reveal when a branch on a removal path keeps a single child: after the removal phase
+ *     (Legacy: removals before upserts; Canonical: upserts first, so inserted keys keep a branch alive) a branch with exactly
+ *     one surviving child c whose node is hashed and on no target's path adds the proof of path ‖ c ‖ 0…0 from depth
+ *     |path ‖ c| on.  Storage tries first; a live account entry is a removal iff its account (the resident one with flag
+ *     bit 1) is empty and its storage root after the block is EMPTY_ROOT_HASH;
+ *   - Legacy only: the storage-root node (both nodes of an extension root, 0x80 for an empty storage) of every account entry
+ *     without storage targets.
+ * Canonical drops every 0x80 node.  An empty block (m = 0) gives the empty map, or with always_include_root the single
+ * entry { state root: root node } ({ EMPTY_ROOT_HASH: 0x80 } for an empty state).  Entries are sorted by hash, without
+ * duplicates: entry i is hashes32[32i ..], rlp[rlp_offset[i] .. rlp_offset[i+1]).  Keys must be strictly ascending
+ * (B200_ERR_UNSORTED).  Not for sharded states (B200_ERR_INVALID_ARG). */
+enum { B200_WITNESS_LEGACY = 0, B200_WITNESS_CANONICAL = 1 };
+typedef struct {
+    uint64_t n;
+    uint8_t *hashes32;     /* [n][32] ascending */
+    uint64_t *rlp_offset;  /* [n+1] */
+    uint8_t *rlp;
+    void *_owner;
+} b200_witness;
+B200_API int32_t b200_dstate_witness(b200_dstate *, const uint8_t *acct_keys32, const b200_account *accts, const uint8_t *acct_flags,
+                                     uint64_t m, const uint8_t *slot_keys32, const uint8_t *values32_be, const uint64_t *seg_offsets,
+                                     int32_t mode, int32_t always_include_root, b200_witness *out);
+B200_API void b200_witness_release(b200_witness *);
 /* b200_dstate_apply with the block already in device memory (every input pointer and d_root32 are device pointers;
  * n_entries = d_seg_offsets[m]); the update records, if wanted, still arrive in host memory. */
 B200_API int32_t b200_dstate_apply_dev(b200_dstate *, const void *d_acct_keys32, const void *d_accts, const void *d_acct_flags,

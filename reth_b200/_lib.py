@@ -62,6 +62,17 @@ class Proofs(C.Structure):
     ]
 
 
+class Witness(C.Structure):
+    """b200_witness (include/b200trie.h)."""
+    _fields_ = [
+        ("n", C.c_uint64),
+        ("hashes32", C.POINTER(C.c_uint8)),
+        ("rlp_offset", C.POINTER(C.c_uint64)),
+        ("rlp", C.POINTER(C.c_uint8)),
+        ("_owner", C.c_void_p),
+    ]
+
+
 class Stats(C.Structure):
     _fields_ = [
         ("leaves_added", C.c_uint64),
@@ -214,6 +225,8 @@ def load():
     sig("b200_dstate_storage_proofs", i32, vp, vp, vp, u64, vp, C.POINTER(Proofs))
     sig("b200_dstate_multiproof", i32, vp, vp, u64, vp, vp, C.POINTER(Proofs), vp, C.POINTER(Proofs))
     sig("b200_proofs_release", None, C.POINTER(Proofs))
+    sig("b200_dstate_witness", i32, vp, vp, vp, vp, u64, vp, vp, vp, i32, i32, C.POINTER(Witness))
+    sig("b200_witness_release", None, C.POINTER(Witness))
     sig("b200_dstate_apply_dev", i32, vp, vp, vp, vp, u64, vp, vp, vp, u64, vp, PU, PU, PU, PU, vp, PS)
     sig("b200_dstate_root", i32, vp, vp)
     sig("b200_dstate_accounts", u64, vp)

@@ -43,10 +43,15 @@ static __device__ void dt_keccak_global(const uint8_t *p, uint32_t len, uint32_t
 
 // Walks target `key` in trie `trie`.  WRITE = false: returns node / byte counts.  WRITE = true: writes the nodes at
 // rlp + byte_base and their start offsets at rlp_offset[node_base ..].
-template <bool WRITE>
+// WITNESS (tk_witness.cuh; node_depth / node_masks unused): an extension and the branch below it are one node of reth's V2
+// proofs (BranchNodeV2 with a key) and TrieWitness records both RLPs (crates/trie/trie/src/witness.rs:328-343), so the
+// branch below a diverging extension is kept too; only nodes whose path is at least `min_len` nibbles long are kept (an
+// extension and its branch by the extension's path: ProofV2Target::with_min_len); WT_ROOT_ONLY stops after the root
+// node (with its branch when it is an extension), WT_FIRST_ONLY after the first node.
+template <bool WRITE, bool WITNESS = false>
 static __device__ void dt_proof_walk(const DTrieDev &t, uint32_t trie, const uint8_t *key, uint32_t &n_nodes, uint64_t &n_bytes,
                                      uint8_t *rlp, uint64_t byte_base, uint64_t *rlp_offset, uint8_t *node_depth, uint32_t *node_masks,
-                                     uint64_t node_base) {
+                                     uint64_t node_base, uint32_t min_len = 0, uint32_t stop = 0) {
     n_nodes = 0;
     n_bytes = 0;
     uint32_t cur = t.troot[trie];
@@ -56,13 +61,16 @@ static __device__ void dt_proof_walk(const DTrieDev &t, uint32_t trie, const uin
     auto begin_node = [&](uint32_t len, int depth, uint32_t masks = 0) {
         if (WRITE) {
             rlp_offset[node_base + n_nodes] = byte_base + n_bytes;
-            node_depth[node_base + n_nodes] = (uint8_t)depth;
-            node_masks[node_base + n_nodes] = masks;
+            if (!WITNESS) {
+                node_depth[node_base + n_nodes] = (uint8_t)depth;
+                node_masks[node_base + n_nodes] = masks;
+            }
         }
         n_nodes++;
         n_bytes += len;
     };
     if (cur == DT_NONE) {  // empty trie: the proof is the empty string (EMPTY_STRING_CODE), proof.rs:121-126
+        if (WITNESS && min_len) return;
         if (WRITE) rlp[byte_base] = 0x80;
         begin_node(1, 0);
         return;
@@ -74,6 +82,7 @@ static __device__ void dt_proof_walk(const DTrieDev &t, uint32_t trie, const uin
             load32_nc(t.lkey + 32 * (uint64_t)x, k);
             const uint8_t *val = t.lval + (uint64_t)t.val_stride * x;
             const uint8_t *sr = t.lsroot ? t.lsroot + 32 * (uint64_t)x : nullptr;
+            if (WITNESS && (uint32_t)(pd + 1) < min_len) return;
             CountBuf cb{0};
             uint32_t len = t.account ? encode_leaf<CountBuf, true>(cb, k, pd, val, sr, t.err) : encode_leaf<CountBuf, false>(cb, k, pd, val, nullptr, t.err);
             if (WRITE) {
@@ -94,7 +103,10 @@ static __device__ void dt_proof_walk(const DTrieDev &t, uint32_t trie, const uin
         const uint32_t masks = ((uint32_t)mk.z << 16) | mk.y;
         const bool ext = pd + 1 < d;
         const bool matches = dt_lcp(key, nk, (uint32_t)(pd + 1), (uint32_t)d) == (uint32_t)d;
-        if (ext) {  // the extension node sits at a prefix of the key (we got here); the branch only if its nibbles match
+        if (WITNESS && !(ext ? (uint32_t)(pd + 1) >= min_len : (uint32_t)d >= min_len)) {
+            // above the wanted depth: walk on without keeping the node
+            if (!matches) return;
+        } else if (ext) {  // the extension node sits at a prefix of the key (we got here); the branch only if its nibbles match
             uint32_t m = (uint32_t)(d - (pd + 1)), hp_len = 1 + (m >> 1), path_str = hp_len == 1 ? 1 : 1 + hp_len;
             uint32_t clen = blen >= 32 ? 33 : blen;
             uint32_t epayload = path_str + clen, elen = list_header_len(epayload) + epayload;
@@ -104,7 +116,9 @@ static __device__ void dt_proof_walk(const DTrieDev &t, uint32_t trie, const uin
                 // thread-local buffer otherwise
                 uint8_t *ext_at = rlp + byte_base + n_bytes;
                 uint8_t tmp[544];
-                uint8_t *br_at = matches ? ext_at + elen : tmp;
+                // (WT_FIRST_ONLY keeps the extension alone: its branch was not counted, whatever the key's nibbles)
+                const bool keep_br = WITNESS ? !(stop & WT_FIRST_ONLY) : matches;
+                uint8_t *br_at = keep_br ? ext_at + elen : tmp;
                 LinBuf br{br_at, 0};
                 dt_put_branch<false>(br, t, v, payload);
                 uint32_t child[8] = {0, 0, 0, 0, 0, 0, 0, 0};
@@ -115,14 +129,21 @@ static __device__ void dt_proof_walk(const DTrieDev &t, uint32_t trie, const uin
                 encode_extension(lb, nk, (uint32_t)(pd + 1), (uint32_t)d, child, blen >= 32 ? 0u : blen);
             }
             begin_node(elen, pd + 1);
-            if (!matches) return;
-            begin_node(blen, d, masks);
+            if (WITNESS) {
+                if (stop & WT_FIRST_ONLY) return;
+                begin_node(blen, d);
+                if (!matches || (stop & (WT_ROOT_ONLY | WT_FIRST_ONLY))) return;
+            } else {
+                if (!matches) return;
+                begin_node(blen, d, masks);
+            }
         } else {
             if (WRITE) {
                 LinBuf br{rlp + byte_base + n_bytes, 0};
                 dt_put_branch<false>(br, t, v, payload);
             }
             begin_node(blen, d, masks);
+            if (WITNESS && (stop & (WT_ROOT_ONLY | WT_FIRST_ONLY))) return;
         }
         pd = d;
         cur = t.nchild[16 * (uint64_t)v + dt_nib(key, (uint32_t)d)];

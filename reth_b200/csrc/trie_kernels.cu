@@ -38,5 +38,6 @@ namespace b200 {
 #include "tk_dstate.cuh"
 #include "tk_proofs.cuh"
 #include "tk_dtrie_launchers.cuh"
+#include "tk_witness.cuh"
 
 }  // namespace b200

@@ -272,6 +272,48 @@ cudaError_t launch_dt_target_tries(const uint64_t *seg_offsets, uint64_t n_accou
                                    uint32_t *trie_of_target, cudaStream_t st);
 cudaError_t launch_dt_find_leaf(const DTrieDev &t, const uint8_t *key, uint32_t *out, uint64_t n_copies, cudaStream_t st);
 
+// ------------------------------------------------------------------------------------------------ witness (tk_witness.cuh)
+constexpr uint32_t WT_ROOT_ONLY = 1, WT_FIRST_ONLY = 2;  // dt_proof_walk stops: after the root node / after the first node kept
+constexpr uint8_t WF_WIPED = 1, WF_EMPTIED = 2;          // storage trie flags: wiped by the block / every leaf removed
+// target meta (u16): low byte min_len (nodes on shorter paths are skipped), then the stop bits; WM_SKIP = no node
+constexpr uint16_t WM_ROOT_ONLY = WT_ROOT_ONLY << 8, WM_FIRST_ONLY = WT_FIRST_ONLY << 8, WM_SKIP = 0x8000;
+struct WitnessMarks {       // per-call scratch of one arena
+    uint32_t *gone;         // [ncap] bit c: every leaf below child c is removed
+    uint32_t *seen;         // [ncap] bit c: a target walks through child c; bit 16 + c: an inserted key does (Canonical)
+    uint32_t *list;         // branches that lost a child, [0, *n_list)
+    uint32_t *n_list;
+    uint8_t *trie_flags;    // storage forest only, [account leaf capacity]: WF_*
+};
+cudaError_t launch_wt_accounts(const DTrieDev &ta, const DTrieDev &ts, const uint8_t *keys, const uint8_t *flags, uint64_t m,
+                               uint32_t *leaf_of, uint8_t *trie_flags, cudaStream_t st);
+cudaError_t launch_wt_slots(const DTrieDev &ts, const WitnessMarks &w, const uint64_t *seg_offsets, uint64_t m, const uint32_t *leaf_of,
+                            const uint8_t *flags, const uint8_t *keys, const uint8_t *vals, uint64_t n, int canonical,
+                            uint32_t *trie_of_target, uint8_t *nonzero, cudaStream_t st);
+cudaError_t launch_wt_account_walk(const DTrieDev &ta, const DTrieDev &ts, const WitnessMarks &w, const uint8_t *keys, const uint8_t *accts,
+                                   const uint8_t *flags, const uint64_t *seg_offsets, uint64_t m, const uint32_t *leaf_of,
+                                   const uint8_t *trie_flags, const uint8_t *nonzero, int canonical, uint32_t *root_trie,
+                                   uint16_t *root_meta, cudaStream_t st);
+cudaError_t launch_wt_reveal(const DTrieDev &t, const WitnessMarks &w, uint32_t max_list, int canonical, uint32_t *out_trie,
+                             uint8_t *out_keys, uint16_t *out_meta, uint32_t *n_out, cudaStream_t st);
+cudaError_t launch_wt_wipe_roots(const DTrieDev &ts, const uint32_t *leaf_of, const uint8_t *trie_flags, uint64_t m, bool write,
+                                 uint32_t *queue, uint32_t *n_queue, uint32_t *n_out, uint32_t *out_trie, uint8_t *out_keys, cudaStream_t st);
+cudaError_t launch_wt_wipe_round(const DTrieDev &ts, uint32_t *queue, uint32_t lo, uint32_t hi, uint32_t *n_queue, uint32_t *n_leaves,
+                                 cudaStream_t st);
+cudaError_t launch_wt_wipe_leaves(const DTrieDev &ts, const uint32_t *queue, uint32_t n, uint32_t *n_out, uint32_t *out_trie,
+                                  uint8_t *out_keys, cudaStream_t st);
+cudaError_t launch_wt_clear(const DTrieDev &t, const WitnessMarks &w, const uint32_t *trie_of, const uint8_t *keys, uint64_t n,
+                            const uint32_t *leaf_of, uint8_t *trie_flags, cudaStream_t st);
+cudaError_t launch_wt_proof_sizes(const DTrieDev &t, const uint32_t *trie_of, const uint8_t *keys, const uint16_t *meta, uint64_t n_fixed,
+                                  const uint32_t *n_extra, uint64_t n_max, uint32_t *node_count, uint64_t *byte_count, cudaStream_t st);
+cudaError_t launch_wt_proof_write(const DTrieDev &t, const uint32_t *trie_of, const uint8_t *keys, const uint16_t *meta, uint64_t n_fixed,
+                                  const uint32_t *n_extra, uint64_t n_max, const uint64_t *node_base, const uint64_t *byte_base,
+                                  uint64_t node_shift, uint64_t byte_shift, uint8_t *rlp, uint64_t *rlp_offset, cudaStream_t st);
+cudaError_t launch_wt_unique(const uint8_t *sorted32, const uint32_t *perm, const uint64_t *rlp_offset, const uint8_t *rlp, uint64_t n,
+                             int drop_empty, uint32_t *keep, uint64_t *kept_bytes, cudaStream_t st);
+cudaError_t launch_wt_gather(const uint8_t *sorted32, const uint32_t *perm, const uint64_t *rlp_offset, const uint8_t *rlp, uint64_t n,
+                             const uint32_t *keep, const uint32_t *pos, const uint64_t *byte_pos, uint8_t *out_hash, uint64_t *out_offset,
+                             uint8_t *out_rlp, cudaStream_t st);
+
 cudaError_t launch_dt_restructure_fused(const DTrieDev &t, const uint32_t *trie_of_key, const uint8_t *keys, const uint8_t *vals,
                                         const uint8_t *flags, const uint8_t *sroots, uint32_t m, uint8_t *kind, uint32_t *leaf_of,
                                         uint32_t *list_a, uint32_t *list_b, uint8_t *defer, uint32_t *idx_a, uint32_t *idx_b,

@@ -10,7 +10,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from ._lib import B200Error, FrontierEntry, Proofs, Stats, Updates
+from ._lib import B200Error, FrontierEntry, Proofs, Stats, Updates, Witness
 
 ACCOUNT_DTYPE = np.dtype([("nonce", "<u8"), ("balance", "u1", (32,)), ("code_hash", "u1", (32,))])
 KECCAK_EMPTY = bytes.fromhex("c5d2460186f7233c927e7db2dcc703c0e500b653ca82273b7bfad8045d85a470")
@@ -901,6 +901,39 @@ class DynamicState:
                         bm[kn[:depth]] = (masks >> 16, masks & 0xFFFF)
             out["storages"][a] = {"root": sroots[i].tobytes(), "subtree": sub, "branch_node_masks": bm}
         return out
+
+    def witness(self, acct_keys, accounts, flags, slot_keys, values, seg_offsets, mode: str = "legacy",
+                always_include_root_node: bool = False) -> dict:
+        """Execution witness of one block given in the `apply` layout, against the state as it is (the state does not
+        change): {keccak(node): node RLP} (TrieWitness::compute; mode "legacy" or "canonical", see include/b200trie.h)."""
+        modes = {"legacy": 0, "canonical": 1}
+        if mode not in modes:
+            raise ValueError(f"mode must be one of {sorted(modes)}")
+        acct_keys = _np(acct_keys).reshape(-1, 32)
+        m = len(acct_keys)
+        accounts = np.ascontiguousarray(accounts, ACCOUNT_DTYPE)
+        fl = None if flags is None else _np(np.asarray(flags, dtype=np.uint8))
+        slot_keys = _np(slot_keys).reshape(-1, 32)
+        values = _np(values).reshape(-1, 32)
+        seg_offsets = _np(seg_offsets, np.uint64)
+        if len(seg_offsets) != m + 1:
+            raise ValueError("seg_offsets must have m+1 entries")
+        if (m and int(seg_offsets[m]) != len(slot_keys)) or len(values) != len(slot_keys):
+            raise ValueError("seg_offsets[m] must equal the number of slot rows (keys and values)")
+        w = Witness()
+        self.engine._check(self.engine.lib.b200_dstate_witness(
+            self.handle, _ptr(acct_keys), _ptr(accounts), _ptr(fl), m, _ptr(slot_keys), _ptr(values), _ptr(seg_offsets),
+            modes[mode], 1 if always_include_root_node else 0, C.byref(w)))
+        try:
+            n = int(w.n)
+            if not n:
+                return {}
+            hashes = np.ctypeslib.as_array(w.hashes32, (n * 32,)).tobytes()
+            ro = np.ctypeslib.as_array(w.rlp_offset, (n + 1,))
+            blob = np.ctypeslib.as_array(w.rlp, (max(int(ro[n]), 1),)).tobytes()
+            return {hashes[32 * i:32 * i + 32]: blob[int(ro[i]):int(ro[i + 1])] for i in range(n)}
+        finally:
+            self.engine.lib.b200_witness_release(C.byref(w))
 
     def account_proofs(self, acct_keys) -> list:
         """-> for every target hashed address the list of node RLPs from the root down (Proof::account_proof)."""

@@ -401,8 +401,9 @@ class DynamicStateRoot:
     def root(self) -> bytes:
         return self.ds.root()
 
-    def commit(self, post) -> Tuple[bytes, TrieUpdates]:
-        """post: HashedPostState -> (root, TrieUpdates of the block)."""
+    def _block(self, post, destroyed_slots: bool):
+        """post: HashedPostState -> (touched keys, the b200_dstate_apply arrays).  destroyed_slots: keep the slot entries
+        of a destroyed account (the witness proves them; an apply ignores them)."""
         from .engine import DynamicState as DS
         touched = sorted(set(post.accounts) | set(post.storages))
         m = len(touched)
@@ -415,7 +416,11 @@ class DynamicStateRoot:
             if k in post.accounts:
                 a = post.accounts[k]
                 if a is None:
-                    offs.append(len(sk))  # destroyed: flags 0, its slots (if any) are irrelevant
+                    if destroyed_slots and hs is not None:
+                        for s, v in sorted(hs.storage.items()):
+                            sk.append(s)
+                            sv.append(int(v).to_bytes(32, "big"))
+                    offs.append(len(sk))  # destroyed: flags 0, its storage is wiped
                     continue
                 flags[i] = DS.EXISTS
                 accts[i]["nonce"] = a.nonce
@@ -432,9 +437,13 @@ class DynamicStateRoot:
             offs.append(len(sk))
         skeys = np.frombuffer(b"".join(sk), np.uint8).reshape(-1, 32) if sk else np.zeros((0, 32), np.uint8)
         svals = np.frombuffer(b"".join(sv), np.uint8).reshape(-1, 32) if sv else np.zeros((0, 32), np.uint8)
+        return touched, (keys, accts, flags, skeys, svals, np.array(offs, np.uint64))
+
+    def commit(self, post) -> Tuple[bytes, TrieUpdates]:
+        """post: HashedPostState -> (root, TrieUpdates of the block)."""
+        touched, block = self._block(post, destroyed_slots=False)
         try:
-            root, au, ar, su, sr, deleted = self.ds.apply(keys, accts, flags, skeys, svals, np.array(offs, np.uint64),
-                                                          want_updates=True)
+            root, au, ar, su, sr, deleted = self.ds.apply(*block, want_updates=True)
         except Exception as e:  # noqa: BLE001
             raise StateRootError(str(e)) from e
         upd = TrieUpdates()
@@ -448,6 +457,27 @@ class DynamicStateRoot:
             st = StorageTrieUpdates(bool(deleted[i]), per_entry.get(i, {}), removed_per_entry.get(i, set()))
             upd.insert_storage_updates(k, st)
         return root, upd
+
+    def witness(self, post, mode: str = "legacy", always_include_root_node: bool = False) -> Dict[bytes, bytes]:
+        """TrieWitness::compute(post) against the state as it is (crates/trie/trie/src/witness.rs): {keccak(node): node RLP}
+        of every trie node a stateless client needs to apply `post` to this state.  mode: "legacy" (reth's default) or
+        "canonical" (ExecutionWitnessMode).  The state is not changed; commit the block afterwards.  Raises StateRootError
+        for a storage entry without an account entry (TrieWitnessError::MissingAccount).
+
+        One difference from reth: the block goes through the layout `commit` uses, in which a destroyed account (None)
+        always loses its storage.  reth's HashedPostState can also say "destroyed, storage not wiped" (no `storages` entry
+        marked wiped); TrieWitness then keeps the account's storage root and upserts the default account, which needs
+        other nodes.  Blocks from execution always wipe the storage of a destroyed account, so both give the same map."""
+        for k in post.storages:
+            if k not in post.accounts:
+                raise StateRootError(f"missing account {k.hex()}")
+        _, block = self._block(post, destroyed_slots=True)
+        try:
+            return self.ds.witness(*block, mode=mode, always_include_root_node=always_include_root_node)
+        except ValueError:
+            raise
+        except Exception as e:  # noqa: BLE001
+            raise StateRootError(str(e)) from e
 
     def close(self):
         self.ds.close()
