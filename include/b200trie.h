@@ -49,7 +49,8 @@ typedef enum {
     B200_ERR_OOM = -6,
     B200_ERR_INLINE_HASH_CHILD = -7, /* a <32-byte branch child under a hash_mask bit while retaining updates:
                                         alloy-trie's child_hashes would panic here; unreachable for keccak keys */
-    B200_ERR_NOT_FOUND = -8 /* b200_trie_update: a dirty key is not in the resident trie */
+    B200_ERR_NOT_FOUND = -8, /* b200_trie_update: a dirty key is not in the resident trie */
+    B200_ERR_WITNESS_INCOMPLETE = -9 /* b200_witness_roots (per block): a node the post-block root needs is not in the witness */
 } b200_status;
 
 /* ------------------------------------------------------------------------------------------------ lifecycle */
@@ -590,6 +591,45 @@ B200_API int32_t b200_dstate_witness(b200_dstate *, const uint8_t *acct_keys32, 
                                      uint64_t m, const uint8_t *slot_keys32, const uint8_t *values32_be, const uint64_t *seg_offsets,
                                      int32_t mode, int32_t always_include_root, b200_witness *out);
 B200_API void b200_witness_release(b200_witness *);
+/* Post-block state roots from execution witnesses: stateless validation (reth: DecodedMultiProofV2::from_witness,
+ * crates/trie/common/src/proofs.rs:469-544, revealed into a SparseStateTrie and updated, crates/trie/sparse/src/state.rs).
+ * A batch of n_blocks independent blocks, each with its own parent state root and witness; no b200_dstate is involved.
+ *   witness of block b : nodes block_node_offset[b] .. block_node_offset[b+1]; node i is
+ *                        node_rlp[node_rlp_offset[i] .. node_rlp_offset[i+1]) (ExecutionWitness.state: RLPs only — every
+ *                        node is hashed on the device).  Duplicates and unrelated nodes are allowed; a block only uses its
+ *                        own nodes.
+ *   block b            : account entries block_acct_offset[b] .. block_acct_offset[b+1] in the layout of b200_dstate_apply and
+ *                        with its rules (keys strictly ascending inside a block; seg_offsets [M+1] over all M entries of the
+ *                        call; flag bit 0 clear = destroyed, its slots ignored; bit 1 = account data unchanged; bit 2 = storage
+ *                        wiped first; zero value deletes a slot; an unchanged entry of an absent account is ignored with its
+ *                        slots; a live entry is an upsert, also of an empty account with an empty storage).
+ * Per block (block_status[b], roots32[32b..]; a failed block's root is zeroed, other blocks are unaffected):
+ *   B200_OK                     : the post-block state root.  A block without entries keeps its parent root and needs no node;
+ *                                 a parent root of EMPTY_ROOT_HASH is the empty state and needs no node.
+ *   B200_ERR_WITNESS_INCOMPLETE : a node the computation needs is missing (also: a parent root whose node is missing).
+ *   B200_ERR_INVALID_ARG        : a node reached from the parent root fails one of these checks, and only these are made
+ *                                 (non-minimal RLP, a branch with fewer than two children or an extension above a leaf or an
+ *                                 extension are accepted as they are): bad RLP, trailing
+ *                                 bytes, a branch with a non-empty 17th item, a leaf path that does not end at nibble 64, an
+ *                                 inline child of 32 bytes or more, a hashed child that is not 32 bytes, an account value
+ *                                 that is not a TrieAccount, a storage value that is zero or longer than 32 bytes).  Wins over
+ *                                 INCOMPLETE.
+ * The nodes needed: (a) every node on the path to each account key of the block, and to each slot key of every live storage
+ * trie the block changes and does not wipe (the path ends at the leaf, an empty slot, or a diverging leaf or extension);
+ * (b) every hashed child on no such path that in the post-block trie hangs more than one nibble below its nearest branch
+ * (its encoding changes), except the child of an extension, which is a branch and keeps its hash.  Nothing of a wiped storage
+ * trie is needed.  A missing node of kind (a) or (b) gives B200_ERR_WITNESS_INCOMPLETE, never a wrong root; so does a
+ * missing hashed leaf at depth 64 (two keys sharing 63 nibbles), which the fold cannot represent.  The witness
+ * b200_dstate_witness returns, in either mode, holds every node of kind (a) and (b).
+ * Call-level errors: null pointers, offsets that do not start at 0 or are not monotone (B200_ERR_INVALID_ARG); keys not
+ * strictly ascending inside a block or an entry (B200_ERR_UNSORTED).  Limit: nodes, entries, and revealed items plus entries
+ * each below 2^31-1 per call (B200_ERR_INVALID_ARG). */
+B200_API int32_t b200_witness_roots(b200_ctx *, uint64_t n_blocks, const uint8_t *parent_roots32, const uint8_t *node_rlp,
+                                    const uint64_t *node_rlp_offset /* [N+1] */, const uint64_t *block_node_offset /* [n_blocks+1] */,
+                                    const uint8_t *acct_keys32, const b200_account *accts, const uint8_t *acct_flags /* nullable */,
+                                    const uint64_t *block_acct_offset /* [n_blocks+1] */, const uint8_t *slot_keys32,
+                                    const uint8_t *values32_be, const uint64_t *seg_offsets /* [M+1] */, uint8_t *roots32,
+                                    int32_t *block_status, b200_stats *opt_stats);
 /* b200_dstate_apply with the block already in device memory (every input pointer and d_root32 are device pointers;
  * n_entries = d_seg_offsets[m]); the update records, if wanted, still arrive in host memory. */
 B200_API int32_t b200_dstate_apply_dev(b200_dstate *, const void *d_acct_keys32, const void *d_accts, const void *d_acct_flags,

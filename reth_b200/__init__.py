@@ -10,7 +10,7 @@ from .hashed_state import (Account, HashedPostState, HashedPostStateSorted, Hash
                            TriePrefixSetsMut, unpack_nibbles)
 from .stages import AccountHashingStage, MerkleStage, StageError, StorageHashingStage, Tables  # noqa: F401,E402
 from .trie import (BranchNodeCompact, DynamicStateRoot, ParallelStateRoot, ResidentStateRoot, StateRoot, StateRootError, StateRootProgress,  # noqa: F401,E402
-                   StorageRoot, StorageTrieUpdates, TrieUpdates)
+                   StorageRoot, StorageTrieUpdates, TrieUpdates, stateless_state_root, stateless_state_roots)
 from .sharded import ShardedDynamicStateRoot, sharded_ordered_trie_roots  # noqa: F401,E402
 from .verify import Verifier  # noqa: F401,E402
 from .ordered_root import (OrderedRootError, OrderedTrieRootEncodedBuilder, ordered_trie_root_encoded,  # noqa: F401,E402

@@ -13,7 +13,7 @@ LIB_PATH = os.path.join(_HERE, "libb200trie.so")
 
 # b200_status (include/b200trie.h)
 OK, ERR_NO_DEVICE, ERR_CUDA, ERR_INVALID_ARG, ERR_UNSORTED, ERR_ZERO_VALUE, ERR_OOM, ERR_INLINE_HASH_CHILD, \
-    ERR_NOT_FOUND = (0, -1, -2, -3, -4, -5, -6, -7, -8)
+    ERR_NOT_FOUND, ERR_WITNESS_INCOMPLETE = (0, -1, -2, -3, -4, -5, -6, -7, -8, -9)
 
 
 class B200Error(RuntimeError):
@@ -227,6 +227,7 @@ def load():
     sig("b200_proofs_release", None, C.POINTER(Proofs))
     sig("b200_dstate_witness", i32, vp, vp, vp, vp, u64, vp, vp, vp, i32, i32, C.POINTER(Witness))
     sig("b200_witness_release", None, C.POINTER(Witness))
+    sig("b200_witness_roots", i32, vp, u64, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, PS)
     sig("b200_dstate_apply_dev", i32, vp, vp, vp, vp, u64, vp, vp, vp, u64, vp, PU, PU, PU, PU, vp, PS)
     sig("b200_dstate_root", i32, vp, vp)
     sig("b200_dstate_accounts", u64, vp)

@@ -107,6 +107,8 @@ extern "C" B200_API void b200_destroy(b200_ctx *c) {
                       &c->ord_item, &c->ord_sched, &c->ord_sched2, &c->ord_pos, &c->ord_order};
     for (DevBuf *b : bufs)
         if (b->p) cudaFree(b->p);
+    for (DevBuf &b : c->sl)
+        if (b.p) cudaFree(b.p);
     if (c->pinned_small) cudaFreeHost(c->pinned_small);
     if (c->ev_fork) cudaEventDestroy(c->ev_fork);
     if (c->ev_join) cudaEventDestroy(c->ev_join);
@@ -391,4 +393,5 @@ extern "C" B200_API uint64_t b200_launch_count(const b200_ctx *c) { return c ? c
 #include "eng_witness.inl"
 #include "eng_ordered.inl"
 #include "eng_items.inl"
+#include "eng_stateless.inl"
 #include "eng_comm.inl"

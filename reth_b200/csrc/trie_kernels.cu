@@ -39,5 +39,6 @@ namespace b200 {
 #include "tk_proofs.cuh"
 #include "tk_dtrie_launchers.cuh"
 #include "tk_witness.cuh"
+#include "tk_stateless.cuh"
 
 }  // namespace b200

@@ -314,6 +314,61 @@ cudaError_t launch_wt_gather(const uint8_t *sorted32, const uint32_t *perm, cons
                              const uint32_t *keep, const uint32_t *pos, const uint64_t *byte_pos, uint8_t *out_hash, uint64_t *out_offset,
                              uint8_t *out_rlp, cudaStream_t st);
 
+// ------------------------------------------------------------------------------------------------ stateless roots (tk_stateless.cuh)
+enum : uint32_t { SL_INCOMPLETE = 1u, SL_INVALID = 2u, SL_NONE = 0xFFFFFFFFu };
+enum : int32_t { SL_STATUS_INVALID = -3, SL_STATUS_INCOMPLETE = -9 };  // == B200_ERR_INVALID_ARG, B200_ERR_WITNESS_INCOMPLETE
+enum : uint8_t { SL_LEAF = 0, SL_BLIND = 1, SL_BLIND_BRANCH = 2 };  // item kinds: leaf, hashed child not in the witness (of
+                                                                    // unknown kind / the child of an extension: a branch)
+struct StatelessDev {
+    const uint8_t *rlp;          // witness nodes of all blocks, node i = rlp[rlp_off[i], rlp_off[i+1])
+    const uint64_t *rlp_off;     // [n_nodes + 1]
+    const uint64_t *block_node;  // [n_blocks + 1] nodes of block b
+    const uint8_t *dig_sorted;   // [n_nodes][32] node digests, ascending
+    const uint32_t *dig_perm;    // [n_nodes] node of each sorted digest
+    uint64_t n_nodes;
+    const uint8_t *parent;       // [n_blocks][32]
+    const uint64_t *block_acct;  // [n_blocks + 1] account entries of block b
+    const uint8_t *akeys;        // [m][32]
+    const uint8_t *accts;        // [m] b200_account rows
+    const uint8_t *aflags;       // [m] or null (all plain upserts)
+    const uint64_t *seg;         // [m + 1] slot entries of account entry a
+    const uint8_t *skeys, *svals;  // [n_e][32]
+    uint64_t n_blocks, m, n_e;
+    uint32_t *status;            // [n_blocks] SL_INCOMPLETE | SL_INVALID
+};
+struct SlNode {  // a queued node: trie, path (packed nibbles, zero-padded) and depth, RLP at rlp[off, off + len)
+    uint8_t path[32];
+    uint64_t off;
+    uint32_t len, trie, block, depth;
+};
+struct SlItem {  // leaf (nib 64, value RLP at rlp[off, off + len); len 0: an inserted entry) or blind child (hash at rlp[off])
+    uint8_t key[32];
+    uint64_t off;
+    uint32_t len, trie, block, entry;  // entry: the slot / account entry that updates or inserts it, or SL_NONE
+    uint8_t nib, kind, pad[6];
+};
+cudaError_t launch_sl_seed(const StatelessDev &s, SlNode *q, uint32_t *n_q, cudaStream_t st);
+cudaError_t launch_sl_reveal(const StatelessDev &s, const SlNode *q, uint32_t nq, SlNode *next, uint32_t *n_next, SlItem *items,
+                             uint32_t *n_items, cudaStream_t st);
+cudaError_t launch_sl_sort_key(const SlItem *items, const uint32_t *perm, uint64_t n, int w, uint64_t *keys, uint32_t *idx,
+                               cudaStream_t st);
+cudaError_t launch_sl_gather(const SlItem *items, const uint32_t *perm, uint64_t n, SlItem *out, cudaStream_t st);
+cudaError_t launch_sl_merge(const StatelessDev &s, SlItem *items, uint64_t n_it, uint32_t *dead, uint32_t *ins, uint32_t *lb,
+                            uint32_t *eblock, cudaStream_t st);
+cudaError_t launch_sl_keep(const StatelessDev &s, const SlItem *items, uint64_t n_it, uint32_t *keep, const uint32_t *eblock,
+                           uint32_t *ins, cudaStream_t st);
+cudaError_t launch_sl_totals(const StatelessDev &s, const SlItem *items, uint64_t n_it, const uint32_t *kscan, const uint32_t *iscan,
+                             uint64_t *totals, cudaStream_t st);
+cudaError_t launch_sl_place(const StatelessDev &s, const SlItem *items, uint64_t n_it, const uint32_t *keep, const uint32_t *kscan,
+                            const uint32_t *ins, const uint32_t *iscan, const uint32_t *lb, const uint32_t *eblock, SlItem *fin,
+                            cudaStream_t st);
+cudaError_t launch_sl_segments(const StatelessDev &s, const SlItem *fin, uint64_t n_fin, uint64_t n_sto, uint64_t *sto_offs,
+                               uint64_t *acc_offs, cudaStream_t st);
+cudaError_t launch_sl_sufficiency(const StatelessDev &s, const SlItem *fin, uint64_t n_fin, cudaStream_t st);
+cudaError_t launch_sl_rows(const StatelessDev &s, const SlItem *fin, uint64_t lo, uint64_t hi, uint8_t *keys, uint8_t *nibs,
+                           uint8_t *flags, uint8_t *values, uint8_t *sroots, const uint8_t *sto_roots, cudaStream_t st);
+cudaError_t launch_sl_finish(const StatelessDev &s, const uint8_t *acc_roots, uint8_t *out, cudaStream_t st);
+
 cudaError_t launch_dt_restructure_fused(const DTrieDev &t, const uint32_t *trie_of_key, const uint8_t *keys, const uint8_t *vals,
                                         const uint8_t *flags, const uint8_t *sroots, uint32_t m, uint8_t *kind, uint32_t *leaf_of,
                                         uint32_t *list_a, uint32_t *list_b, uint8_t *defer, uint32_t *idx_a, uint32_t *idx_b,

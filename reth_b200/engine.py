@@ -202,6 +202,19 @@ class Engine:
             return roots, updates_to_records(u, self.lib)
         return roots
 
+    def witness_roots(self, parent_roots, witnesses, blocks):
+        """b200_witness_roots: the post-block state root of every block from its parent root, its execution witness and the
+        block alone.  witnesses[b]: a list of node RLPs or a {hash: rlp} dict (only the RLPs are sent); blocks[b]: the
+        `DynamicState.apply` array tuple (acct_keys, accounts, flags, slot_keys, values, seg_offsets).
+        -> (roots uint8[n, 32], statuses int32[n]): per block OK, ERR_WITNESS_INCOMPLETE or ERR_INVALID_ARG (root zeroed)."""
+        args = witness_batch_arrays(parent_roots, witnesses, blocks)
+        n = args[0]
+        roots = np.zeros((n, 32), np.uint8)
+        status = np.zeros(n, np.int32)
+        s = Stats()
+        self._check(self.lib.b200_witness_roots(self.ctx, n, *(_ptr(a) for a in args[1:]), _ptr(roots), _ptr(status), C.byref(s)))
+        return roots, status
+
     def hash_changesets(self, acct_addresses, storage_addresses, storage_slots) -> dict:
         """b200_hash_changesets: the account / storage changesets of a block range (addresses uint8[na,20]; rows
         (address uint8[ns,20], slot uint8[ns,32]) in changeset order) -> the range's dirty set: unique hashed keys sorted,
@@ -415,6 +428,40 @@ class Engine:
 
     def dev_status(self):
         self._check(self.lib.b200_dev_status(self.ctx))
+
+
+def witness_batch_arrays(parent_roots, witnesses, blocks) -> tuple:
+    """The arguments of b200_witness_roots from n_blocks .. seg_offsets, in ABI order: the parent roots, the RLPs of every
+    witness concatenated (a witness is a list of node RLPs or a {hash: rlp} dict: only the RLPs are sent), and the blocks
+    (`DynamicState.apply` array tuples) concatenated."""
+    n = len(blocks)
+    if len(parent_roots) != n or len(witnesses) != n:
+        raise ValueError("one parent root and one witness per block")
+    parents = _np(np.frombuffer(b"".join(bytes(p) for p in parent_roots), np.uint8) if n else np.zeros(0, np.uint8)).reshape(n, 32)
+    nodes = [bytes(r) for w in witnesses for r in (w.values() if isinstance(w, dict) else w)]
+    block_node = np.cumsum([0] + [len(w) for w in witnesses], dtype=np.uint64)
+    rlp_off = np.cumsum([0] + [len(r) for r in nodes], dtype=np.uint64)
+    rlp = np.frombuffer(b"".join(nodes) or b"\0", np.uint8)
+    keys, accts, flags, skeys, svals, offs, block_acct = [], [], [], [], [], [0], [0]
+    for k, a, f, sk, sv, so in blocks:
+        k = _np(k).reshape(-1, 32)
+        m = len(k)
+        so = _np(so, np.uint64)
+        sk, sv = _np(sk).reshape(-1, 32), _np(sv).reshape(-1, 32)
+        if len(so) != m + 1 or int(so[0]) != 0 or int(so[m]) != len(sk) or len(sv) != len(sk):
+            raise ValueError("seg_offsets must have m+1 entries from 0 to the number of slot rows (keys and values)")
+        keys.append(k)
+        accts.append(np.ascontiguousarray(a, ACCOUNT_DTYPE).reshape(m))
+        flags.append(np.ones(m, np.uint8) if f is None else _np(np.asarray(f, dtype=np.uint8)).reshape(m))
+        skeys.append(sk)
+        svals.append(sv)
+        offs.extend((so[1:] + np.uint64(offs[-1])).tolist())
+        block_acct.append(block_acct[-1] + m)
+    cat = lambda xs, shape, dt: np.ascontiguousarray(np.concatenate(xs)) if xs else np.zeros(shape, dt)
+    keys, accts, flags = cat(keys, (0, 32), np.uint8), cat(accts, 0, ACCOUNT_DTYPE), cat(flags, 0, np.uint8)
+    skeys, svals = cat(skeys, (0, 32), np.uint8), cat(svals, (0, 32), np.uint8)
+    return (n, parents, rlp, rlp_off, block_node, keys, accts, flags, np.array(block_acct, np.uint64), skeys, svals,
+            np.array(offs, np.uint64))
 
 
 def _prefer_bundled_nccl():

@@ -13,6 +13,7 @@ from typing import Dict, List, Optional, Tuple
 
 import numpy as np
 
+from ._lib import ERR_WITNESS_INCOMPLETE
 from .engine import EMPTY_ROOT_HASH, Engine
 from .hashed_state import HashedPostStateSorted, HashedStorageSorted, TriePrefixSets
 
@@ -380,6 +381,45 @@ class ResidentStateRoot:
         self.trie.close()
 
 
+def apply_layout(post, destroyed_slots: bool):
+    """post: HashedPostState -> (touched keys, the b200_dstate_apply arrays).  destroyed_slots: keep the slot entries
+    of a destroyed account (the witness proves them; an apply ignores them)."""
+    from .engine import ACCOUNT_DTYPE, DynamicState as DS
+    touched = sorted(set(post.accounts) | set(post.storages))
+    m = len(touched)
+    keys = np.frombuffer(b"".join(touched), np.uint8).reshape(m, 32) if m else np.zeros((0, 32), np.uint8)
+    accts = np.zeros(m, ACCOUNT_DTYPE)
+    flags = np.zeros(m, np.uint8)
+    sk, sv, offs = [], [], [0]
+    for i, k in enumerate(touched):
+        hs = post.storages.get(k)
+        if k in post.accounts:
+            a = post.accounts[k]
+            if a is None:
+                if destroyed_slots and hs is not None:
+                    for s, v in sorted(hs.storage.items()):
+                        sk.append(s)
+                        sv.append(int(v).to_bytes(32, "big"))
+                offs.append(len(sk))  # destroyed: flags 0, its storage is wiped
+                continue
+            flags[i] = DS.EXISTS
+            accts[i]["nonce"] = a.nonce
+            accts[i]["balance"] = np.frombuffer(int(a.balance).to_bytes(32, "big"), np.uint8)
+            accts[i]["code_hash"] = np.frombuffer(a.code_hash(), np.uint8)
+        else:
+            flags[i] = DS.EXISTS | DS.UNCHANGED  # storage-only change
+        if hs is not None:
+            if hs.wiped:
+                flags[i] |= DS.WIPED
+            for s, v in sorted(hs.storage.items()):
+                sk.append(s)
+                sv.append(int(v).to_bytes(32, "big"))
+        offs.append(len(sk))
+    skeys = np.frombuffer(b"".join(sk), np.uint8).reshape(-1, 32) if sk else np.zeros((0, 32), np.uint8)
+    svals = np.frombuffer(b"".join(sv), np.uint8).reshape(-1, 32) if sv else np.zeros((0, 32), np.uint8)
+    return touched, (keys, accts, flags, skeys, svals, np.array(offs, np.uint64))
+
+
 class DynamicStateRoot:
     """Live-path commitment with the WHOLE hashed state resident in HBM (b200_dstate_*): accounts and every storage trie.
 
@@ -402,42 +442,7 @@ class DynamicStateRoot:
         return self.ds.root()
 
     def _block(self, post, destroyed_slots: bool):
-        """post: HashedPostState -> (touched keys, the b200_dstate_apply arrays).  destroyed_slots: keep the slot entries
-        of a destroyed account (the witness proves them; an apply ignores them)."""
-        from .engine import DynamicState as DS
-        touched = sorted(set(post.accounts) | set(post.storages))
-        m = len(touched)
-        keys = np.frombuffer(b"".join(touched), np.uint8).reshape(m, 32) if m else np.zeros((0, 32), np.uint8)
-        accts = np.zeros(m, self._dtype)
-        flags = np.zeros(m, np.uint8)
-        sk, sv, offs = [], [], [0]
-        for i, k in enumerate(touched):
-            hs = post.storages.get(k)
-            if k in post.accounts:
-                a = post.accounts[k]
-                if a is None:
-                    if destroyed_slots and hs is not None:
-                        for s, v in sorted(hs.storage.items()):
-                            sk.append(s)
-                            sv.append(int(v).to_bytes(32, "big"))
-                    offs.append(len(sk))  # destroyed: flags 0, its storage is wiped
-                    continue
-                flags[i] = DS.EXISTS
-                accts[i]["nonce"] = a.nonce
-                accts[i]["balance"] = np.frombuffer(int(a.balance).to_bytes(32, "big"), np.uint8)
-                accts[i]["code_hash"] = np.frombuffer(a.code_hash(), np.uint8)
-            else:
-                flags[i] = DS.EXISTS | DS.UNCHANGED  # storage-only change
-            if hs is not None:
-                if hs.wiped:
-                    flags[i] |= DS.WIPED
-                for s, v in sorted(hs.storage.items()):
-                    sk.append(s)
-                    sv.append(int(v).to_bytes(32, "big"))
-            offs.append(len(sk))
-        skeys = np.frombuffer(b"".join(sk), np.uint8).reshape(-1, 32) if sk else np.zeros((0, 32), np.uint8)
-        svals = np.frombuffer(b"".join(sv), np.uint8).reshape(-1, 32) if sv else np.zeros((0, 32), np.uint8)
-        return touched, (keys, accts, flags, skeys, svals, np.array(offs, np.uint64))
+        return apply_layout(post, destroyed_slots)
 
     def commit(self, post) -> Tuple[bytes, TrieUpdates]:
         """post: HashedPostState -> (root, TrieUpdates of the block)."""
@@ -481,3 +486,32 @@ class DynamicStateRoot:
 
     def close(self):
         self.ds.close()
+
+
+def stateless_state_roots(engine: Engine, parent_roots, witnesses, posts) -> List[bytes]:
+    """Stateless validation of a batch of blocks (b200_witness_roots): the post-block state root of every block from its
+    parent root, its execution witness (ExecutionWitness.state: a list of node RLPs, or a {hash: rlp} map) and its
+    HashedPostState alone.  Raises StateRootError for a storage entry without an account entry, and for the first block
+    whose witness is incomplete or holds a malformed node (naming the block and the status)."""
+    blocks = []
+    for post in posts:
+        for k in post.storages:
+            if k not in post.accounts:
+                raise StateRootError(f"missing account {k.hex()}")
+        blocks.append(apply_layout(post, destroyed_slots=False)[1])
+    try:
+        roots, statuses = engine.witness_roots(list(parent_roots), list(witnesses), blocks)
+    except ValueError:
+        raise
+    except Exception as e:  # noqa: BLE001
+        raise StateRootError(str(e)) from e
+    for b, st in enumerate(statuses):
+        if st:
+            what = "witness incomplete" if st == ERR_WITNESS_INCOMPLETE else "malformed witness node"
+            raise StateRootError(f"block {b}: {what} (status {int(st)})")
+    return [r.tobytes() for r in roots]
+
+
+def stateless_state_root(engine: Engine, parent_root: bytes, witness, post) -> bytes:
+    """stateless_state_roots for one block."""
+    return stateless_state_roots(engine, [parent_root], [witness], [post])[0]
