@@ -5,6 +5,7 @@
 #include <cstring>
 #include <mutex>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include <cuda_runtime.h>
@@ -12,11 +13,53 @@
 #include "../../include/b200trie.h"
 #include "pinned_pool.h"
 
-// ------------------------------------------------------------------------------------------------ context
+// ------------------------------------------------------------------------------------------------ device memory
+// One block of device memory, charged to the byte counter of its owner (b200_ctx::dev_bytes, or the `bytes` of a trie or
+// state).  Released, and taken off that counter, by reset(), by the destructor, or when a move overwrites it.  An owner
+// declares its counter before the buffers charged to it: members are destroyed in reverse order.  The caller makes sure
+// no queued work still uses a block it releases.  Only grow() allocates.
 struct DevBuf {
     void *p = nullptr;
     size_t cap = 0;
+    uint64_t *owner = nullptr;  // the counter `cap` is charged to
+
+    DevBuf() = default;
+    DevBuf(const DevBuf &) = delete;
+    DevBuf &operator=(const DevBuf &) = delete;
+    DevBuf(DevBuf &&o) noexcept : p(o.p), cap(o.cap), owner(o.owner) {
+        o.p = nullptr;
+        o.cap = 0;
+    }
+    DevBuf &operator=(DevBuf &&o) noexcept {
+        if (this != &o) {
+            reset();
+            std::swap(p, o.p);
+            std::swap(cap, o.cap);
+            owner = o.owner;
+        }
+        return *this;
+    }
+    ~DevBuf() { reset(); }
+    void reset() {
+        if (p) {
+            cudaFree(p);
+            *owner -= cap;
+        }
+        p = nullptr;
+        cap = 0;
+    }
+    // takes over `src`'s block (releasing this one's) and charges it to `counter`: a buffer handed to another owner
+    void take(DevBuf &src, uint64_t *counter) {
+        *this = std::move(src);
+        if (p) {
+            *owner -= cap;
+            *counter += cap;
+        }
+        owner = counter;
+    }
 };
+
+// ------------------------------------------------------------------------------------------------ context
 
 struct b200_ctx {
     int device = 0;
@@ -105,20 +148,38 @@ inline int32_t fail(b200_ctx *c, int32_t code, const char *fmt, ...) {
                         #call, cudaGetErrorString(e__), __FILE__, __LINE__);                                  \
     } while (0)
 
-inline int32_t ensure(b200_ctx *c, DevBuf &b, size_t bytes) {
-    if (bytes <= b.cap) return B200_OK;
-    if (b.p) {
-        CU(cudaStreamSynchronize(c->stream));  // buffer may still be in use by queued work
-        CU(cudaFree(b.p));
-        c->dev_bytes -= b.cap;
-        b.p = nullptr;
-        b.cap = 0;
+// Every device allocation: if `b` holds fewer than `need` bytes, it gets a new block of `want` bytes charged to *counter,
+// filled with the byte `fill` (>= 0) and holding the first `keep` bytes of the old block.  With nothing to keep the old
+// block is released first, so that the two never coexist.  On failure `b` is either unchanged or empty, and every
+// counter matches what is allocated.
+inline int32_t grow(b200_ctx *c, uint64_t *counter, DevBuf &b, size_t need, size_t want, size_t keep = 0, int fill = -1) {
+    if (need <= b.cap) return B200_OK;
+    if (c->phase_timing) fprintf(stderr, "[b200 grow] %zu -> %zu bytes (keep %zu)\n", b.cap, want, keep);
+    if (b.p && !keep) {
+        CU(cudaStreamSynchronize(c->stream));  // the block may still be in use by queued work
+        b.reset();
     }
-    size_t want = bytes + bytes / 8 + 256;  // slack so that slowly growing inputs do not re-allocate every call
-    CU(cudaMalloc(&b.p, want));
-    b.cap = want;
-    c->dev_bytes += want;
+    void *p = nullptr;
+    CU(cudaMalloc(&p, want));
+    DevBuf nb;
+    nb.p = p;
+    nb.cap = want;
+    nb.owner = counter;
+    *counter += want;
+    if (fill >= 0) CU(cudaMemsetAsync(p, fill, want, c->stream));
+    if (b.p) {
+        CU(cudaMemcpyAsync(p, b.p, keep, cudaMemcpyDeviceToDevice, c->stream));
+        CU(cudaStreamSynchronize(c->stream));
+    }
+    b = std::move(nb);
     return B200_OK;
+}
+// size rules: the context's scratch takes 1/8 slack, so that slowly growing inputs do not re-allocate every call;
+// resident tries and arena capacity are sized to fit
+inline size_t ctx_cap(size_t bytes) { return bytes + bytes / 8 + 256; }
+inline int32_t ensure(b200_ctx *c, DevBuf &b, size_t bytes) { return grow(c, &c->dev_bytes, b, bytes, ctx_cap(bytes)); }
+inline int32_t grow_fit(b200_ctx *c, uint64_t *counter, DevBuf &b, size_t bytes, size_t keep = 0, int fill = -1) {
+    return grow(c, counter, b, bytes, bytes + 256, keep, fill);
 }
 #define ENSURE(buf, bytes)                                   \
     do {                                                     \
