@@ -11,14 +11,14 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 FAST = ("not one_million and not pipelined and not reentrancy and not frontier_sharding and not commits_blocks "
-        "and not 200000 and not receipt_and_transaction_shaped and not persistent_waves")
+        "and not 200000 and not receipt_and_transaction_shaped and not persistent_waves and not large_block")
 
 
 def test_cuda_sources_pass_parity_under_cpu_emulation():
     r = subprocess.run([sys.executable, "-m", "pytest", "tests/test_gpu_trie.py", "tests/test_gpu_keccak.py",
                         "tests/test_gpu_host_mirror.py", "tests/test_gpu_dtrie.py", "tests/test_gpu_dstate.py", "tests/test_gpu_proofs.py",
                         "tests/test_gpu_zz_ordered_roots.py", "tests/test_gpu_zz_table_rows_device.py", "tests/test_gpu_level_classes.py",
-                        "-m", "gpu", "--emu", "-q", "-x", "-k", FAST,
+                        "tests/test_gpu_leaf_widths.py", "-m", "gpu", "--emu", "-q", "-x", "-k", FAST,
                         "-p", "no:cacheprovider"],
                        cwd=ROOT, capture_output=True, text=True, timeout=1500)
     tail = (r.stdout + r.stderr)[-3000:]
