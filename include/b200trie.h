@@ -630,6 +630,19 @@ B200_API int32_t b200_witness_roots(b200_ctx *, uint64_t n_blocks, const uint8_t
                                     const uint64_t *block_acct_offset /* [n_blocks+1] */, const uint8_t *slot_keys32,
                                     const uint8_t *values32_be, const uint64_t *seg_offsets /* [M+1] */, uint8_t *roots32,
                                     int32_t *block_status, b200_stats *opt_stats);
+/* Post-block state roots of a batch of candidate blocks, each applied on its own to the state as it is (siblings, not a
+ * chain); the state does not change (reth: StateRootProvider::state_root(hashed_state) on the latest state — payload
+ * validation, payload building, sibling payloads; a chain of uncommitted blocks is one block with their merged entries).
+ * Block b: account entries block_acct_offset[b] .. block_acct_offset[b+1], in the layout of b200_dstate_apply and with its
+ * rules (flags bit 0/1/2, zero value deletes, seg_offsets [M+1] over all M entries of the call).  roots32[32b..] = the root
+ * b200_dstate_apply of that block alone would return.  A block without entries gives the current root.  There is no per-block
+ * status: the resident state holds every node a block needs.  Call-level errors as b200_witness_roots (B200_ERR_INVALID_ARG
+ * for null pointers, offsets that do not start at 0 or are not monotone, and the limits; B200_ERR_UNSORTED); a sharded state
+ * gives B200_ERR_INVALID_ARG.  No TrieUpdates: the block that is kept gets them from b200_dstate_apply. */
+B200_API int32_t b200_dstate_overlay_roots(b200_dstate *, uint64_t n_blocks, const uint8_t *acct_keys32, const b200_account *accts,
+                                           const uint8_t *acct_flags /* nullable */, const uint64_t *block_acct_offset /* [n_blocks+1] */,
+                                           const uint8_t *slot_keys32, const uint8_t *values32_be, const uint64_t *seg_offsets /* [M+1] */,
+                                           uint8_t *roots32, b200_stats *opt_stats);
 /* b200_dstate_apply with the block already in device memory (every input pointer and d_root32 are device pointers;
  * n_entries = d_seg_offsets[m]); the update records, if wanted, still arrive in host memory. */
 B200_API int32_t b200_dstate_apply_dev(b200_dstate *, const void *d_acct_keys32, const void *d_accts, const void *d_acct_flags,

@@ -1,0 +1,189 @@
+// tk_overlay.cuh — post-block state roots of candidate blocks on top of the resident state, read-only
+// (b200_dstate_overlay_roots, eng_overlay.inl).  Part of the single translation unit trie_kernels.cu (included inside
+// namespace b200, after tk_stateless.cuh: it produces the items that the stateless tail sorts, merges and folds).
+//
+// reth's StateRootProvider::state_root(hashed_state) on the latest state.  Every block of the batch is its own
+// computation against the arenas as they are: the tries are revealed from the arenas, level by level, along the paths of
+// the block's keys, into the items of tk_stateless.cuh — leaves (full key, value in the encoding a witness carries) and
+// the hashes of the branches no key reaches (kind SL_BLIND_BRANCH at the branch's own path, so the fold re-creates the
+// extension above it).  Trie ids as in the stateless path: storage trie of account entry a = a, account trie of block
+// b = m + b.  A queued branch carries the contiguous range of its trie's targets that pass through it: the block's
+// sorted account keys, or the entry's sorted slot keys.  Nothing is written into the arenas.
+
+// nibbles [from, to) of `key` against those of `path`: -1 / 0 / 1
+__device__ __forceinline__ int ov_cmp_nibbles(const uint8_t *key, const uint8_t *path, uint32_t from, uint32_t to) {
+    for (uint32_t i = from; i < to; i++) {
+        const uint32_t a = sl_nib(key, i), b = sl_nib(path, i);
+        if (a != b) return a < b ? -1 : 1;
+    }
+    return 0;
+}
+// first target in [lo, hi) whose nibbles [from, to) compare above `bound` against `path` (ascending keys that share the
+// first `from` nibbles)
+__device__ __forceinline__ uint32_t ov_first_above(const uint8_t *keys, uint32_t lo, uint32_t hi, const uint8_t *path, uint32_t from,
+                                                   uint32_t to, int bound) {
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (ov_cmp_nibbles(keys + 32 * (uint64_t)mid, path, from, to) <= bound) lo = mid + 1;
+        else hi = mid;
+    }
+    return lo;
+}
+
+// The value of leaf x as its trie's leaf carries it: rlp(TrieAccount) with the leaf's storage root, or rlp(U256).
+__device__ uint32_t ov_leaf_value(const DTrieDev &t, uint32_t x, uint8_t *out) {
+    const uint8_t *v = t.lval + (uint64_t)t.val_stride * x;
+    uint32_t n = 0;
+    auto u256 = [&](const uint8_t *be, uint32_t width) {  // big-endian integer of `width` bytes, leading zeros stripped
+        uint32_t z = 0;
+        while (z < width && be[z] == 0) z++;
+        if (z == width) out[n++] = 0x80;
+        else if (z == width - 1 && be[z] < 0x80) out[n++] = be[z];
+        else {
+            out[n++] = (uint8_t)(0x80 + width - z);
+            for (uint32_t k = z; k < width; k++) out[n++] = be[k];
+        }
+    };
+    if (!t.account) {
+        u256(v, 32);
+        return n;
+    }
+    const b200_account_dev &a = *reinterpret_cast<const b200_account_dev *>(v);
+    uint8_t nonce[8];
+    for (int k = 0; k < 8; k++) nonce[k] = (uint8_t)(a.nonce >> (8 * (7 - k)));
+    n = 2;  // [0xf8, payload]: the payload holds two 33-byte hashes
+    u256(nonce, 8);
+    u256(a.balance_be, 32);
+    out[n++] = 0xa0;
+    for (int k = 0; k < 32; k++) out[n++] = t.lsroot[32 * (uint64_t)x + k];
+    out[n++] = 0xa0;
+    for (int k = 0; k < 32; k++) out[n++] = a.code_hash[k];
+    out[0] = 0xf8;
+    out[1] = (uint8_t)(n - 2);
+    return n;
+}
+
+__device__ __forceinline__ SlItem &ov_item(SlItem *items, uint32_t *n_items, uint32_t trie, uint32_t block, uint32_t &idx) {
+    idx = atomicAdd(n_items, 1u);
+    SlItem &it = items[idx];
+    it.off = (uint64_t)OV_STRIDE * idx;
+    it.trie = trie;
+    it.block = block;
+    it.entry = SL_NONE;
+    return it;
+}
+
+// Child word w of a branch at depth pd (-1: w is the root word of its trie) with the targets [lo, hi) that pass through
+// the child's slot: a leaf is an item; a branch is queued with the targets that share its whole path, or, when none do and
+// its RLP is at least 32 bytes, is an item holding the hash of the branch itself (under an implicit extension the
+// reference its parent holds is the extension's, so the branch is re-hashed).  A branch shorter than 32 bytes has no hash
+// form: it is queued with its (possibly empty) range and its children become items.
+__device__ void ov_word(const DTrieDev &t, const StatelessDev &s, uint32_t w, int pd, uint32_t trie, uint32_t block, uint32_t lo,
+                        uint32_t hi, OvNode *next, uint32_t *n_next, SlItem *items, uint32_t *n_items, uint8_t *vals) {
+    uint32_t idx;
+    if (w & DT_LEAF) {
+        const uint32_t x = w & ~DT_LEAF;
+        SlItem &it = ov_item(items, n_items, trie, block, idx);
+        for (int k = 0; k < 32; k++) it.key[k] = t.lkey[32 * (uint64_t)x + k];
+        it.len = ov_leaf_value(t, x, vals + it.off);
+        it.nib = 64;
+        it.kind = SL_LEAF;
+        return;
+    }
+    const uint32_t d = t.ndepth[w];
+    const uint8_t *nk = t.nkey + 32 * (uint64_t)w;
+    const bool ext = (int)d > pd + 1;
+    if (ext && lo < hi) {  // the targets that diverge inside the extension do not reach the branch
+        const uint8_t *keys = trie >= s.m ? s.akeys : s.skeys;
+        lo = ov_first_above(keys, lo, hi, nk, (uint32_t)(pd + 1), d, -1);
+        hi = ov_first_above(keys, lo, hi, nk, (uint32_t)(pd + 1), d, 0);
+    }
+    uint32_t sm, tm, hm;
+    const uint32_t payload = dt_branch_payload<false>(t, w, sm, tm, hm), blen = list_header_len(payload) + payload;
+    if (lo < hi || blen < 32) {
+        OvNode &e = next[atomicAdd(n_next, 1u)];
+        e.node = w;
+        e.trie = trie;
+        e.block = block;
+        e.lo = lo;
+        e.hi = hi;
+        return;
+    }
+    SlItem &it = ov_item(items, n_items, trie, block, idx);
+    uint8_t *h = vals + it.off;
+    if (ext) {
+        uint8_t br[544];
+        LinBuf lb{br, 0};
+        dt_put_branch<false>(lb, t, w, payload);
+        uint32_t dig[8];
+        dt_keccak_global(br, blen, dig);
+        for (int k = 0; k < 32; k++) h[k] = (uint8_t)(dig[k >> 2] >> (8 * (k & 3)));
+    } else {
+        for (int k = 0; k < 32; k++) h[k] = t.nref[32 * (uint64_t)w + k];
+    }
+    for (int k = 0; k < 32; k++) it.key[k] = 0;
+    for (uint32_t k = 0; k < d; k++) sl_set_nib(it.key, k, sl_nib(nk, k));
+    it.len = 32;
+    it.nib = (uint8_t)d;
+    it.kind = SL_BLIND_BRANCH;
+}
+
+// Threads [0, n_blocks): the account root of every block with entries (and the block's parent root for the finish: the
+// current root).  Threads [n_blocks, n_blocks + m): the storage root of every entry that is live, not wiped, has slots and
+// whose account exists with a non-empty storage trie — so the storage tries are revealed at the same levels as the
+// account tries.
+__global__ void ov_seed_kernel(DTrieDev ta, DTrieDev ts, StatelessDev s, const uint8_t *root, uint8_t *parent, OvNode *q,
+                               uint32_t *n_q, SlItem *items, uint32_t *n_items, uint8_t *vals) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < s.n_blocks) {
+        for (int k = 0; k < 32; k++) parent[32 * i + k] = root[k];
+        const uint32_t lo = (uint32_t)s.block_acct[i], hi = (uint32_t)s.block_acct[i + 1], w = ta.troot[0];
+        if (lo < hi && w != DT_NONE) ov_word(ta, s, w, -1, (uint32_t)(s.m + i), (uint32_t)i, lo, hi, q, n_q, items, n_items, vals);
+        return;
+    }
+    const uint64_t a = i - s.n_blocks;
+    if (a >= s.m) return;
+    const uint32_t fl = sl_flags(s, a);
+    if (!(fl & 1) || (fl & 4) || s.seg[a + 1] == s.seg[a]) return;
+    const DtLoc loc = dt_descend(ta, 0, s.akeys + 32 * a);
+    if (!loc.found) return;
+    const uint32_t w = ts.troot[loc.child & ~DT_LEAF];
+    if (w != DT_NONE)
+        ov_word(ts, s, w, -1, (uint32_t)a, sl_block_of_entry(s, a), (uint32_t)s.seg[a], (uint32_t)s.seg[a + 1], q, n_q, items, n_items,
+                vals);
+}
+
+// One level: every queued branch splits its targets by the nibble at its depth and hands each child its part.
+__global__ void ov_reveal_kernel(DTrieDev ta, DTrieDev ts, StatelessDev s, const OvNode *q, uint32_t nq, OvNode *next, uint32_t *n_next,
+                                 SlItem *items, uint32_t *n_items, uint8_t *vals) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= nq) return;
+    const OvNode e = q[i];
+    const bool account = e.trie >= s.m;
+    const DTrieDev &t = account ? ta : ts;
+    const uint8_t *keys = account ? s.akeys : s.skeys;
+    const uint32_t d = t.ndepth[e.node];
+    const uint32_t *ch = t.nchild + 16 * (uint64_t)e.node;
+    uint32_t lo = e.lo;
+    for (uint32_t c = 0; c < 16; c++) {
+        uint32_t hi = lo, top = e.hi;  // first target in [lo, e.hi) whose nibble d is above c
+        while (hi < top) {
+            const uint32_t mid = (hi + top) >> 1;
+            if (sl_nib(keys + 32 * (uint64_t)mid, d) <= c) hi = mid + 1;
+            else top = mid;
+        }
+        if (ch[c] != DT_NONE) ov_word(t, s, ch[c], (int)d, e.trie, e.block, lo, hi, next, n_next, items, n_items, vals);
+        lo = hi;
+    }
+}
+
+cudaError_t launch_ov_seed(const DTrieDev &ta, const DTrieDev &ts, const StatelessDev &s, const uint8_t *root, uint8_t *parent, OvNode *q,
+                           uint32_t *n_q, SlItem *items, uint32_t *n_items, uint8_t *vals, cudaStream_t st) {
+    ov_seed_kernel<<<blocks_for(s.n_blocks + s.m, 128), 128, 0, st>>>(ta, ts, s, root, parent, q, n_q, items, n_items, vals);
+    return cudaGetLastError();
+}
+cudaError_t launch_ov_reveal(const DTrieDev &ta, const DTrieDev &ts, const StatelessDev &s, const OvNode *q, uint32_t nq, OvNode *next,
+                             uint32_t *n_next, SlItem *items, uint32_t *n_items, uint8_t *vals, cudaStream_t st) {
+    ov_reveal_kernel<<<blocks_for(nq, 128), 128, 0, st>>>(ta, ts, s, q, nq, next, n_next, items, n_items, vals);
+    return cudaGetLastError();
+}

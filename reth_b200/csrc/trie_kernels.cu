@@ -40,5 +40,6 @@ namespace b200 {
 #include "tk_dtrie_launchers.cuh"
 #include "tk_witness.cuh"
 #include "tk_stateless.cuh"
+#include "tk_overlay.cuh"
 
 }  // namespace b200

@@ -369,6 +369,16 @@ cudaError_t launch_sl_rows(const StatelessDev &s, const SlItem *fin, uint64_t lo
                            uint8_t *flags, uint8_t *values, uint8_t *sroots, const uint8_t *sto_roots, cudaStream_t st);
 cudaError_t launch_sl_finish(const StatelessDev &s, const uint8_t *acc_roots, uint8_t *out, cudaStream_t st);
 
+// ------------------------------------------------------------------------------------------------ overlay roots (tk_overlay.cuh)
+struct OvNode {  // a queued branch of an arena: trie id of the call, block, and the targets [lo, hi) that pass through it
+    uint32_t node, trie, block, lo, hi;
+};
+constexpr uint32_t OV_STRIDE = 112;  // value bytes of item i at OV_STRIDE * i: rlp(TrieAccount) (<= 110), rlp(U256) (<= 33), a hash
+cudaError_t launch_ov_seed(const DTrieDev &ta, const DTrieDev &ts, const StatelessDev &s, const uint8_t *root, uint8_t *parent, OvNode *q,
+                           uint32_t *n_q, SlItem *items, uint32_t *n_items, uint8_t *vals, cudaStream_t st);
+cudaError_t launch_ov_reveal(const DTrieDev &ta, const DTrieDev &ts, const StatelessDev &s, const OvNode *q, uint32_t nq, OvNode *next,
+                             uint32_t *n_next, SlItem *items, uint32_t *n_items, uint8_t *vals, cudaStream_t st);
+
 cudaError_t launch_dt_restructure_fused(const DTrieDev &t, const uint32_t *trie_of_key, const uint8_t *keys, const uint8_t *vals,
                                         const uint8_t *flags, const uint8_t *sroots, uint32_t m, uint8_t *kind, uint32_t *leaf_of,
                                         uint32_t *list_a, uint32_t *list_b, uint8_t *defer, uint32_t *idx_a, uint32_t *idx_b,

@@ -442,6 +442,12 @@ def witness_batch_arrays(parent_roots, witnesses, blocks) -> tuple:
     block_node = np.cumsum([0] + [len(w) for w in witnesses], dtype=np.uint64)
     rlp_off = np.cumsum([0] + [len(r) for r in nodes], dtype=np.uint64)
     rlp = np.frombuffer(b"".join(nodes) or b"\0", np.uint8)
+    return (n, parents, rlp, rlp_off, block_node) + block_batch_arrays(blocks)
+
+
+def block_batch_arrays(blocks) -> tuple:
+    """A batch of blocks (`DynamicState.apply` array tuples) concatenated, in ABI order: acct_keys, accts, acct_flags,
+    block_acct_offset, slot_keys, values, seg_offsets (b200_witness_roots, b200_dstate_overlay_roots)."""
     keys, accts, flags, skeys, svals, offs, block_acct = [], [], [], [], [], [0], [0]
     for k, a, f, sk, sv, so in blocks:
         k = _np(k).reshape(-1, 32)
@@ -460,8 +466,7 @@ def witness_batch_arrays(parent_roots, witnesses, blocks) -> tuple:
     cat = lambda xs, shape, dt: np.ascontiguousarray(np.concatenate(xs)) if xs else np.zeros(shape, dt)
     keys, accts, flags = cat(keys, (0, 32), np.uint8), cat(accts, 0, ACCOUNT_DTYPE), cat(flags, 0, np.uint8)
     skeys, svals = cat(skeys, (0, 32), np.uint8), cat(svals, (0, 32), np.uint8)
-    return (n, parents, rlp, rlp_off, block_node, keys, accts, flags, np.array(block_acct, np.uint64), skeys, svals,
-            np.array(offs, np.uint64))
+    return keys, accts, flags, np.array(block_acct, np.uint64), skeys, svals, np.array(offs, np.uint64)
 
 
 def _prefer_bundled_nccl():
@@ -981,6 +986,17 @@ class DynamicState:
             return {hashes[32 * i:32 * i + 32]: blob[int(ro[i]):int(ro[i + 1])] for i in range(n)}
         finally:
             self.engine.lib.b200_witness_release(C.byref(w))
+
+    def overlay_roots(self, blocks) -> list:
+        """b200_dstate_overlay_roots: the root `apply` of each block alone would return, against the state as it is (the
+        state does not change).  blocks: `apply` array tuples (acct_keys, accounts, flags, slot_keys, values, seg_offsets),
+        siblings on the current state, not a chain.  -> a list of 32-byte roots."""
+        args = block_batch_arrays(blocks)
+        n = len(blocks)
+        roots = np.zeros((max(n, 1), 32), np.uint8)
+        s = Stats()
+        self.engine._check(self.engine.lib.b200_dstate_overlay_roots(self.handle, n, *(_ptr(a) for a in args), _ptr(roots), C.byref(s)))
+        return [roots[b].tobytes() for b in range(n)]
 
     def account_proofs(self, acct_keys) -> list:
         """-> for every target hashed address the list of node RLPs from the root down (Proof::account_proof)."""

@@ -484,6 +484,25 @@ class DynamicStateRoot:
         except Exception as e:  # noqa: BLE001
             raise StateRootError(str(e)) from e
 
+    def overlay_roots(self, posts) -> List[bytes]:
+        """StateRootProvider::state_root(hashed_state) on the latest state (crates/storage/storage-api/src/trie.rs) for a batch
+        of candidate blocks, in one device call (b200_dstate_overlay_roots): the root `commit` of each post alone would
+        return, with the state left as it is — to validate a payload, or to finish every payload built on this parent, before
+        `commit` keeps one of them.  The posts are siblings on the current state, not a chain.  A chain of uncommitted blocks
+        is one post merged with HashedPostState.extend, as MemoryOverlayStateProvider merges its in-memory blocks
+        (crates/chain-state/src/memory_overlay.rs).  No TrieUpdates: `commit` returns those of the block that is kept."""
+        blocks = [self._block(post, destroyed_slots=False)[1] for post in posts]
+        try:
+            return self.ds.overlay_roots(blocks)
+        except ValueError:
+            raise
+        except Exception as e:  # noqa: BLE001
+            raise StateRootError(str(e)) from e
+
+    def overlay_root(self, post) -> bytes:
+        """overlay_roots for one post: the root `commit(post)` would return, without changing the state."""
+        return self.overlay_roots([post])[0]
+
     def close(self):
         self.ds.close()
 

@@ -1,0 +1,161 @@
+#!/usr/bin/env python3
+"""Cost of post-block roots of candidate blocks on top of the resident state (b200_dstate_overlay_roots), against the routes
+it replaces, on the C3-shaped state.
+
+    python -m pytest tests/test_gpu_overlay.py -m gpu -q      # correctness first
+    python tools/overlay_bench.py --accounts 1000000 --slots 16 --touch 2000 --siblings 16
+
+Seeds the state of tools/witness_bench.py (--accounts accounts x --slots slots) as a resident b200_dstate and makes
+--siblings blocks of its 2 000-account shape, all on that one parent.  Times, with the state unchanged: the overlay of the
+first block; the overlay of all siblings in one call; b200_dstate_witness (Legacy) + b200_witness_roots of the first block.
+Then times b200_dstate_apply over a chain of fresh blocks of the same shape (an apply changes the state, so every rep
+applies a new block); the first apply is the first sibling, and its root must equal the overlay's.  Every sibling's overlay
+root must equal its witness_roots root on the unchanged state.  CUDA-event time on the call's stream and host-call time
+of the C ABI call alone (inputs packed beforehand), after warm-ups, median / min / max over --reps.  Counts per call:
+kernel launches (b200_launch_count), device-to-host read-backs and host-to-device copies from a separate torch.profiler
+run of one call.  Reads the card's name, power limit and SM clock in the same run.  Prints one JSON line."""
+import argparse
+import ctypes as C
+import json
+import os
+import sys
+import time
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+from tools.stateless_bench import card, spread  # noqa: E402
+from tools.witness_bench import block_arrays, make_block, make_state  # noqa: E402
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--accounts", type=int, default=1_000_000)
+    ap.add_argument("--slots", type=int, default=16)
+    ap.add_argument("--touch", type=int, default=2000)
+    ap.add_argument("--slot-writes", type=int, default=10)
+    ap.add_argument("--siblings", type=int, default=16)
+    ap.add_argument("--reps", type=int, default=10)
+    ap.add_argument("--warmup", type=int, default=3)
+    args = ap.parse_args()
+    import torch
+
+    from reth_b200 import DynamicState, Engine
+    from reth_b200._lib import Stats, Witness
+    from reth_b200.engine import _ptr, block_batch_arrays, witness_batch_arrays
+    out = {"card": card()}
+    eng = Engine(0)
+    keys, accs, skeys, svals, offs = make_state(np.random.default_rng(3), args.accounts, args.slots)
+    ds = DynamicState.create(eng, keys, accs, skeys, svals, offs)
+    parent = ds.root()
+    rng = np.random.default_rng(77)
+    arrays = [block_arrays(make_block(rng, keys, skeys, offs, args.touch, args.slot_writes)) for _ in range(args.siblings)]
+    out.update({"accounts": args.accounts, "slots": args.accounts * args.slots, "block_accounts": len(arrays[0][0]),
+                "block_slot_entries": len(arrays[0][3]), "siblings": args.siblings})
+    stream = torch.cuda.current_stream()
+    eng.set_stream(stream.cuda_stream)
+    ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+
+    def measure(call, reps=args.reps, before=None):
+        l0 = eng.launch_count()
+        if before:
+            before()
+        call()
+        launches = eng.launch_count() - l0
+        for _ in range(args.warmup):
+            if before:
+                before()
+            call()
+        dev, host = [], []
+        for _ in range(reps):
+            if before:
+                before()
+            torch.cuda.synchronize()
+            ev0.record(stream)
+            t0 = time.perf_counter()
+            call()
+            host.append((time.perf_counter() - t0) * 1e3)
+            ev1.record(stream)
+            ev1.synchronize()
+            dev.append(ev0.elapsed_time(ev1))
+        from torch.profiler import ProfilerActivity, profile
+        if before:
+            before()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            call()
+            torch.cuda.synchronize()
+        names = [e.name for e in prof.events()]
+        return {"device_ms": spread(dev), "host_call_ms": spread(host), "launches": launches,
+                "readbacks_dtoh": sum(1 for n in names if "DtoH" in n), "copies_htod": sum(1 for n in names if "HtoD" in n)}
+
+    # ---- overlay: one block, then every sibling in one call
+    def overlay_case(nb):
+        packed = block_batch_arrays(arrays[:nb])
+        roots = np.zeros((nb, 32), np.uint8)
+        s = Stats()
+
+        def call():
+            eng._check(eng.lib.b200_dstate_overlay_roots(ds.handle, nb, *(_ptr(x) for x in packed), _ptr(roots), C.byref(s)))
+        r = measure(call)
+        r["blocks"] = nb
+        r["host_call_ms_per_block"] = round(r["host_call_ms"]["median"] / nb, 3)
+        return r, [x.tobytes() for x in roots]
+
+    out["overlay_one"], one_root = overlay_case(1)
+    out["overlay_batch"], batch_roots = overlay_case(args.siblings)
+    assert batch_roots[0] == one_root[0] and ds.root() == parent
+
+    # ---- the read-only route it replaces: witness, then witness_roots, of the first block
+    a0 = arrays[0]
+    wit_roots = []
+    for a in arrays:
+        w = ds.witness(*a, mode="legacy")
+        r, st = eng.witness_roots([parent], [w], [a])
+        assert int(st[0]) == 0
+        wit_roots.append(r[0].tobytes())
+    assert wit_roots == batch_roots, "overlay root differs from the witness_roots root"
+    w0 = ds.witness(*a0, mode="legacy")
+    packed_w = witness_batch_arrays([parent], [w0], [a0])
+    roots_w, status_w = np.zeros((1, 32), np.uint8), np.zeros(1, np.int32)
+
+    def witness_route():
+        w = Witness()
+        eng._check(eng.lib.b200_dstate_witness(ds.handle, _ptr(a0[0]), _ptr(a0[1]), _ptr(a0[2]), len(a0[0]), _ptr(a0[3]),
+                                               _ptr(a0[4]), _ptr(a0[5]), 0, 0, C.byref(w)))
+        eng.lib.b200_witness_release(C.byref(w))  # (the witness reaches the host: a caller would pass it on as it is)
+        eng._check(eng.lib.b200_witness_roots(eng.ctx, 1, *(_ptr(x) for x in packed_w[1:]), _ptr(roots_w), _ptr(status_w),
+                                              C.byref(Stats())))
+    out["witness_plus_witness_roots"] = measure(witness_route)
+    assert roots_w[0].tobytes() == one_root[0] and ds.root() == parent
+
+    # ---- apply: the first sibling, then a chain of fresh blocks of the same shape
+    root0 = ds.apply(*a0)
+    assert root0 == one_root[0], "overlay root differs from the apply"
+    chain = iter(block_arrays(make_block(rng, keys, skeys, offs, args.touch, args.slot_writes))
+                 for _ in range(args.warmup + args.reps + 2))
+    cur = {}
+    root = np.zeros(32, np.uint8)
+
+    def next_block():
+        cur["a"] = next(chain)
+
+    def apply_call():
+        a = cur["a"]
+        eng._check(eng.lib.b200_dstate_apply(ds.handle, _ptr(a[0]), _ptr(a[1]), _ptr(a[2]), len(a[0]), _ptr(a[3]), _ptr(a[4]),
+                                             _ptr(a[5]), _ptr(root), None, None, None, None, None, C.byref(Stats())))
+    out["apply_chain"] = measure(apply_call, before=next_block)
+    out["apply_chain"]["note"] = "every rep applies a fresh block of the same shape on top of the previous one"
+    o1, ob = out["overlay_one"]["device_ms"]["median"], out["overlay_batch"]["device_ms"]["median"]
+    out["ratios"] = {"witness_route_over_overlay": round(out["witness_plus_witness_roots"]["device_ms"]["median"] / o1, 2),
+                     "batch_over_one": round(ob / o1, 2),
+                     "overlay_over_apply": round(o1 / out["apply_chain"]["device_ms"]["median"], 2)}
+    out["card_after"] = card()
+    print(json.dumps(out))
+    ds.close()
+    eng.close()
+
+
+if __name__ == "__main__":
+    main()
