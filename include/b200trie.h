@@ -638,11 +638,33 @@ B200_API int32_t b200_witness_roots(b200_ctx *, uint64_t n_blocks, const uint8_t
  * b200_dstate_apply of that block alone would return.  A block without entries gives the current root.  There is no per-block
  * status: the resident state holds every node a block needs.  Call-level errors as b200_witness_roots (B200_ERR_INVALID_ARG
  * for null pointers, offsets that do not start at 0 or are not monotone, and the limits; B200_ERR_UNSORTED); a sharded state
- * gives B200_ERR_INVALID_ARG.  No TrieUpdates: the block that is kept gets them from b200_dstate_apply. */
+ * gives B200_ERR_INVALID_ARG.  The same as b200_dstate_overlay_roots_with_updates without outputs. */
 B200_API int32_t b200_dstate_overlay_roots(b200_dstate *, uint64_t n_blocks, const uint8_t *acct_keys32, const b200_account *accts,
                                            const uint8_t *acct_flags /* nullable */, const uint64_t *block_acct_offset /* [n_blocks+1] */,
                                            const uint8_t *slot_keys32, const uint8_t *values32_be, const uint64_t *seg_offsets /* [M+1] */,
                                            uint8_t *roots32, b200_stats *opt_stats);
+/* b200_dstate_overlay_roots plus the TrieUpdates of every block (reth: StateRoot::overlay_root_with_updates, what
+ * state_root_with_updates(hashed_state) returns); the state still does not change.  Inputs, roots and call-level errors as
+ * b200_dstate_overlay_roots.  Outputs, all nullable, as b200_dstate_apply's: account records with trie_id = block index;
+ * storage records with trie_id = account entry index over the whole call (block b owns entries block_acct_offset[b] ..
+ * [b+1]); opt_storage_deleted[M].  On error every list is released and zeroed, and opt_storage_deleted is zeroed (all M
+ * bytes, once block_acct_offset has passed its checks; before that M is not known and the array is left as it is); with no
+ * entries every requested list is valid and empty.  opt_stats covers the whole call, both folds included.  The records follow reth's walker (TrieWalker + HashBuilder):
+ *   updated : every stored branch the block's keys pass through, rebuilt — also on the path of a key that changes nothing
+ *             (the delete of an absent slot, an ignored unchanged entry); unchanged siblings stay hashes and get no record;
+ *   removed : every stored branch on such a path that is no longer a stored branch at the same path afterwards; masks 0, no
+ *             hashes, the empty path never; a path that is also updated (same trie) is not removed (updates.rs:160-167);
+ *   storage_deleted[i] : exactly b200_dstate_apply's flag — entry i's account exists and is destroyed, or exists and its
+ *             storage is wiped.
+ * Where a block changes the structure, the records can differ from b200_dstate_apply's of the same block in records that
+ * restate a stored node as it is (both describe the same tables after the block). */
+B200_API int32_t b200_dstate_overlay_roots_with_updates(b200_dstate *, uint64_t n_blocks, const uint8_t *acct_keys32,
+                                                        const b200_account *accts, const uint8_t *acct_flags /* nullable */,
+                                                        const uint64_t *block_acct_offset /* [n_blocks+1] */, const uint8_t *slot_keys32,
+                                                        const uint8_t *values32_be, const uint64_t *seg_offsets /* [M+1] */,
+                                                        uint8_t *roots32, b200_updates *opt_acct_updated, b200_updates *opt_acct_removed,
+                                                        b200_updates *opt_storage_updated, b200_updates *opt_storage_removed,
+                                                        uint8_t *opt_storage_deleted /* [M] */, b200_stats *opt_stats);
 /* b200_dstate_apply with the block already in device memory (every input pointer and d_root32 are device pointers;
  * n_entries = d_seg_offsets[m]); the update records, if wanted, still arrive in host memory. */
 B200_API int32_t b200_dstate_apply_dev(b200_dstate *, const void *d_acct_keys32, const void *d_accts, const void *d_acct_flags,

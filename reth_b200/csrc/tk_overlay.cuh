@@ -9,6 +9,11 @@
 // extension above it).  Trie ids as in the stateless path: storage trie of account entry a = a, account trie of block
 // b = m + b.  A queued branch carries the contiguous range of its trie's targets that pass through it: the block's
 // sorted account keys, or the entry's sorted slot keys.  Nothing is written into the arenas.
+//
+// With TrieUpdates (b200_dstate_overlay_roots_with_updates) a hash item also carries its parent's tree-mask bit as the arena
+// holds it (reth's CursorSubNode::tree_flag: the branch is stored), so that the fold rebuilds the stored records of the
+// branches on the keys' paths; and every stored branch the reveal queues (not at the empty path) is a removed-node
+// candidate, dropped later when the fold stores a record at the same path.
 
 // nibbles [from, to) of `key` against those of `path`: -1 / 0 / 1
 __device__ __forceinline__ int ov_cmp_nibbles(const uint8_t *key, const uint8_t *path, uint32_t from, uint32_t to) {
@@ -70,16 +75,18 @@ __device__ __forceinline__ SlItem &ov_item(SlItem *items, uint32_t *n_items, uin
     it.trie = trie;
     it.block = block;
     it.entry = SL_NONE;
+    it.tree = 0;
     return it;
 }
 
 // Child word w of a branch at depth pd (-1: w is the root word of its trie) with the targets [lo, hi) that pass through
-// the child's slot: a leaf is an item; a branch is queued with the targets that share its whole path, or, when none do and
-// its RLP is at least 32 bytes, is an item holding the hash of the branch itself (under an implicit extension the
-// reference its parent holds is the extension's, so the branch is re-hashed).  A branch shorter than 32 bytes has no hash
-// form: it is queued with its (possibly empty) range and its children become items.
-__device__ void ov_word(const DTrieDev &t, const StatelessDev &s, uint32_t w, int pd, uint32_t trie, uint32_t block, uint32_t lo,
-                        uint32_t hi, OvNode *next, uint32_t *n_next, SlItem *items, uint32_t *n_items, uint8_t *vals) {
+// the child's slot, and the parent's tree-mask bit for that slot (`tree`; for a root word ov_root_tree): a leaf is an
+// item; a branch is queued with the targets that share its whole path, or, when none do and its RLP is at least 32 bytes,
+// is an item holding the hash of the branch itself (under an implicit extension the reference its parent holds is the
+// extension's, so the branch is re-hashed).  A branch shorter than 32 bytes has no hash form: it is queued with its
+// (possibly empty) range and its children become items.
+__device__ void ov_word(const DTrieDev &t, const StatelessDev &s, uint32_t w, int pd, uint32_t tree, uint32_t trie, uint32_t block,
+                        uint32_t lo, uint32_t hi, OvNode *next, uint32_t *n_next, SlItem *items, uint32_t *n_items, uint8_t *vals) {
     uint32_t idx;
     if (w & DT_LEAF) {
         const uint32_t x = w & ~DT_LEAF;
@@ -126,36 +133,46 @@ __device__ void ov_word(const DTrieDev &t, const StatelessDev &s, uint32_t w, in
     it.len = 32;
     it.nib = (uint8_t)d;
     it.kind = SL_BLIND_BRANCH;
+    it.tree = (uint8_t)tree;
+}
+
+// A root word has no parent branch, but when every key leaves the extension above it, the fold builds a new branch above
+// it whose tree-mask bit for it is what the arena's parent would hold: whether the branch itself is stored.
+__device__ __forceinline__ uint32_t ov_root_tree(const DTrieDev &t, uint32_t w) {
+    return !(w & DT_LEAF) && (t.nmeta[w] & META_STORED) ? 1u : 0u;
 }
 
 // Threads [0, n_blocks): the account root of every block with entries (and the block's parent root for the finish: the
 // current root).  Threads [n_blocks, n_blocks + m): the storage root of every entry that is live, not wiped, has slots and
 // whose account exists with a non-empty storage trie — so the storage tries are revealed at the same levels as the
-// account tries.
+// account tries.  found (nullable): found[a] = entry a's account is in the account arena.
 __global__ void ov_seed_kernel(DTrieDev ta, DTrieDev ts, StatelessDev s, const uint8_t *root, uint8_t *parent, OvNode *q,
-                               uint32_t *n_q, SlItem *items, uint32_t *n_items, uint8_t *vals) {
+                               uint32_t *n_q, SlItem *items, uint32_t *n_items, uint8_t *vals, uint8_t *found) {
     const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < s.n_blocks) {
         for (int k = 0; k < 32; k++) parent[32 * i + k] = root[k];
         const uint32_t lo = (uint32_t)s.block_acct[i], hi = (uint32_t)s.block_acct[i + 1], w = ta.troot[0];
-        if (lo < hi && w != DT_NONE) ov_word(ta, s, w, -1, (uint32_t)(s.m + i), (uint32_t)i, lo, hi, q, n_q, items, n_items, vals);
+        if (lo < hi && w != DT_NONE) ov_word(ta, s, w, -1, ov_root_tree(ta, w), (uint32_t)(s.m + i), (uint32_t)i, lo, hi, q, n_q, items, n_items, vals);
         return;
     }
     const uint64_t a = i - s.n_blocks;
     if (a >= s.m) return;
     const uint32_t fl = sl_flags(s, a);
-    if (!(fl & 1) || (fl & 4) || s.seg[a + 1] == s.seg[a]) return;
+    const bool reveal = (fl & 1) && !(fl & 4) && s.seg[a + 1] != s.seg[a];
+    if (!reveal && !found) return;
     const DtLoc loc = dt_descend(ta, 0, s.akeys + 32 * a);
-    if (!loc.found) return;
+    if (found) found[a] = loc.found ? 1 : 0;
+    if (!reveal || !loc.found) return;
     const uint32_t w = ts.troot[loc.child & ~DT_LEAF];
     if (w != DT_NONE)
-        ov_word(ts, s, w, -1, (uint32_t)a, sl_block_of_entry(s, a), (uint32_t)s.seg[a], (uint32_t)s.seg[a + 1], q, n_q, items, n_items,
+        ov_word(ts, s, w, -1, ov_root_tree(ts, w), (uint32_t)a, sl_block_of_entry(s, a), (uint32_t)s.seg[a], (uint32_t)s.seg[a + 1], q, n_q, items, n_items,
                 vals);
 }
 
-// One level: every queued branch splits its targets by the nibble at its depth and hands each child its part.
+// One level: every queued branch splits its targets by the nibble at its depth and hands each child its part; a stored one
+// (not at the empty path) is a removed-node candidate when rm keeps them.
 __global__ void ov_reveal_kernel(DTrieDev ta, DTrieDev ts, StatelessDev s, const OvNode *q, uint32_t nq, OvNode *next, uint32_t *n_next,
-                                 SlItem *items, uint32_t *n_items, uint8_t *vals) {
+                                 SlItem *items, uint32_t *n_items, uint8_t *vals, OvRemoved rm) {
     const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= nq) return;
     const OvNode e = q[i];
@@ -164,6 +181,13 @@ __global__ void ov_reveal_kernel(DTrieDev ta, DTrieDev ts, StatelessDev s, const
     const uint8_t *keys = account ? s.akeys : s.skeys;
     const uint32_t d = t.ndepth[e.node];
     const uint32_t *ch = t.nchild + 16 * (uint64_t)e.node;
+    const uint32_t tree_mask = t.nmasks[e.node].y;
+    if (rm.acc && (t.nmeta[e.node] & META_STORED) && d != 0) {
+        uint32_t *cand = account ? rm.acc : rm.sto;
+        const uint32_t k = atomicAdd(account ? rm.n_acc : rm.n_sto, 1u);
+        cand[2 * k] = e.trie;
+        cand[2 * k + 1] = e.node;
+    }
     uint32_t lo = e.lo;
     for (uint32_t c = 0; c < 16; c++) {
         uint32_t hi = lo, top = e.hi;  // first target in [lo, e.hi) whose nibble d is above c
@@ -172,18 +196,37 @@ __global__ void ov_reveal_kernel(DTrieDev ta, DTrieDev ts, StatelessDev s, const
             if (sl_nib(keys + 32 * (uint64_t)mid, d) <= c) hi = mid + 1;
             else top = mid;
         }
-        if (ch[c] != DT_NONE) ov_word(t, s, ch[c], (int)d, e.trie, e.block, lo, hi, next, n_next, items, n_items, vals);
+        if (ch[c] != DT_NONE) ov_word(t, s, ch[c], (int)d, (tree_mask >> c) & 1u, e.trie, e.block, lo, hi, next, n_next, items, n_items, vals);
         lo = hi;
     }
 }
 
+// Candidate k -> (trie id - trie_base, path length, packed path): the rows of the removed records (as dt_removed_paths_kernel)
+__global__ void ov_removed_paths_kernel(DTrieDev t, const uint32_t *__restrict__ cand, uint32_t n, uint32_t trie_base,
+                                        uint8_t *__restrict__ path_len, uint8_t *__restrict__ path_packed, uint32_t *__restrict__ trie_id) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint32_t v = cand[2 * i + 1], d = t.nmasks[v].w;
+    const uint8_t *key = t.nkey + 32 * (uint64_t)v;
+    uint8_t *pp = path_packed + 32 * (uint64_t)i;
+    for (uint32_t b = 0; b < 32; b++) pp[b] = (uint8_t)(2 * b + 1 < d ? key[b] : (2 * b < d ? (key[b] & 0xF0) : 0));
+    path_len[i] = (uint8_t)d;
+    trie_id[i] = cand[2 * i] - trie_base;
+}
+
 cudaError_t launch_ov_seed(const DTrieDev &ta, const DTrieDev &ts, const StatelessDev &s, const uint8_t *root, uint8_t *parent, OvNode *q,
-                           uint32_t *n_q, SlItem *items, uint32_t *n_items, uint8_t *vals, cudaStream_t st) {
-    ov_seed_kernel<<<blocks_for(s.n_blocks + s.m, 128), 128, 0, st>>>(ta, ts, s, root, parent, q, n_q, items, n_items, vals);
+                           uint32_t *n_q, SlItem *items, uint32_t *n_items, uint8_t *vals, uint8_t *found, cudaStream_t st) {
+    ov_seed_kernel<<<blocks_for(s.n_blocks + s.m, 128), 128, 0, st>>>(ta, ts, s, root, parent, q, n_q, items, n_items, vals, found);
     return cudaGetLastError();
 }
 cudaError_t launch_ov_reveal(const DTrieDev &ta, const DTrieDev &ts, const StatelessDev &s, const OvNode *q, uint32_t nq, OvNode *next,
-                             uint32_t *n_next, SlItem *items, uint32_t *n_items, uint8_t *vals, cudaStream_t st) {
-    ov_reveal_kernel<<<blocks_for(nq, 128), 128, 0, st>>>(ta, ts, s, q, nq, next, n_next, items, n_items, vals);
+                             uint32_t *n_next, SlItem *items, uint32_t *n_items, uint8_t *vals, OvRemoved rm, cudaStream_t st) {
+    ov_reveal_kernel<<<blocks_for(nq, 128), 128, 0, st>>>(ta, ts, s, q, nq, next, n_next, items, n_items, vals, rm);
+    return cudaGetLastError();
+}
+cudaError_t launch_ov_removed_paths(const DTrieDev &t, const uint32_t *cand, uint32_t n, uint32_t trie_base, uint8_t *path_len,
+                                    uint8_t *path_packed, uint32_t *trie_id, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    ov_removed_paths_kernel<<<blocks_for(n, 128), 128, 0, st>>>(t, cand, n, trie_base, path_len, path_packed, trie_id);
     return cudaGetLastError();
 }

@@ -146,6 +146,7 @@ __device__ __forceinline__ void sl_emit(SlItem *items, uint32_t *n_items, const 
     it.entry = SL_NONE;
     it.nib = (uint8_t)nib;
     it.kind = (uint8_t)kind;
+    it.tree = 0;  // (a witness node does not say whether a hashed child is stored)
 }
 
 // The root node of every block with entries and a non-empty parent state starts the walk; a missing one: incomplete.
@@ -359,6 +360,7 @@ __global__ void sl_place_kernel(StatelessDev s, const SlItem *items, uint64_t n_
         f.entry = slot ? (uint32_t)j : (uint32_t)a;
         f.nib = 64;
         f.kind = SL_LEAF;
+        f.tree = 0;
     }
 }
 // Segment offsets of the two forests: storage segment a (m of them), account segment b (n_blocks), from the final items.
@@ -391,7 +393,7 @@ __global__ void sl_sufficiency_kernel(StatelessDev s, const SlItem *fin, uint64_
     }
     if ((int)fin[i].nib > pd + 1) atomicOr(s.status + fin[i].block, SL_INCOMPLETE);
 }
-// Fold inputs of final items [lo, hi): keys, nibbles, flags (0), and the value rows — storage: U256 (entry or decoded leaf);
+// Fold inputs of final items [lo, hi): keys, nibbles, flags (the item's tree bit: children_are_in_trie), and the value rows — storage: U256 (entry or decoded leaf);
 // accounts: b200_account (entry unless "unchanged", else the decoded leaf) and the storage root (the new root when the entry
 // changes the storage or the account is new, else the leaf's).  A blind item's row starts with its hash.
 __global__ void sl_rows_kernel(StatelessDev s, const SlItem *fin, uint64_t lo, uint64_t hi, uint8_t *keys, uint8_t *nibs, uint8_t *flags,
@@ -402,7 +404,7 @@ __global__ void sl_rows_kernel(StatelessDev s, const SlItem *fin, uint64_t lo, u
     const uint64_t r = i - lo;
     for (int k = 0; k < 32; k++) keys[32 * r + k] = f.key[k];
     nibs[r] = f.nib;
-    flags[r] = 0;
+    flags[r] = f.tree;
     const bool account = sroots != nullptr;
     uint8_t *row = values + (account ? 72 : 32) * r;
     if (f.kind != SL_LEAF) {

@@ -345,7 +345,9 @@ struct SlItem {  // leaf (nib 64, value RLP at rlp[off, off + len); len 0: an in
     uint8_t key[32];
     uint64_t off;
     uint32_t len, trie, block, entry;  // entry: the slot / account entry that updates or inserts it, or SL_NONE
-    uint8_t nib, kind, pad[6];
+    uint8_t nib, kind;
+    uint8_t tree;  // a hash item whose branch is stored (children_are_in_trie: its parent's tree-mask bit); 0 otherwise
+    uint8_t pad[5];
 };
 cudaError_t launch_sl_seed(const StatelessDev &s, SlNode *q, uint32_t *n_q, cudaStream_t st);
 cudaError_t launch_sl_reveal(const StatelessDev &s, const SlNode *q, uint32_t nq, SlNode *next, uint32_t *n_next, SlItem *items,
@@ -374,10 +376,18 @@ struct OvNode {  // a queued branch of an arena: trie id of the call, block, and
     uint32_t node, trie, block, lo, hi;
 };
 constexpr uint32_t OV_STRIDE = 112;  // value bytes of item i at OV_STRIDE * i: rlp(TrieAccount) (<= 110), rlp(U256) (<= 33), a hash
+// Removed-node candidates of an overlay with TrieUpdates: (trie id of the call, arena node) of every stored branch that the
+// reveal queues, account tries and storage tries apart; null lists: none are kept (the root-only call).
+struct OvRemoved {
+    uint32_t *acc, *sto;      // [2][..] pairs
+    uint32_t *n_acc, *n_sto;  // counts
+};
 cudaError_t launch_ov_seed(const DTrieDev &ta, const DTrieDev &ts, const StatelessDev &s, const uint8_t *root, uint8_t *parent, OvNode *q,
-                           uint32_t *n_q, SlItem *items, uint32_t *n_items, uint8_t *vals, cudaStream_t st);
+                           uint32_t *n_q, SlItem *items, uint32_t *n_items, uint8_t *vals, uint8_t *found, cudaStream_t st);
 cudaError_t launch_ov_reveal(const DTrieDev &ta, const DTrieDev &ts, const StatelessDev &s, const OvNode *q, uint32_t nq, OvNode *next,
-                             uint32_t *n_next, SlItem *items, uint32_t *n_items, uint8_t *vals, cudaStream_t st);
+                             uint32_t *n_next, SlItem *items, uint32_t *n_items, uint8_t *vals, OvRemoved rm, cudaStream_t st);
+cudaError_t launch_ov_removed_paths(const DTrieDev &t, const uint32_t *cand, uint32_t n, uint32_t trie_base, uint8_t *path_len,
+                                    uint8_t *path_packed, uint32_t *trie_id, cudaStream_t st);
 
 cudaError_t launch_dt_restructure_fused(const DTrieDev &t, const uint32_t *trie_of_key, const uint8_t *keys, const uint8_t *vals,
                                         const uint8_t *flags, const uint8_t *sroots, uint32_t m, uint8_t *kind, uint32_t *leaf_of,

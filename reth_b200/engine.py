@@ -987,16 +987,35 @@ class DynamicState:
         finally:
             self.engine.lib.b200_witness_release(C.byref(w))
 
-    def overlay_roots(self, blocks) -> list:
+    def overlay_roots(self, blocks, want_updates: bool = False) -> list:
         """b200_dstate_overlay_roots: the root `apply` of each block alone would return, against the state as it is (the
         state does not change).  blocks: `apply` array tuples (acct_keys, accounts, flags, slot_keys, values, seg_offsets),
-        siblings on the current state, not a chain.  -> a list of 32-byte roots."""
+        siblings on the current state, not a chain.  -> a list of 32-byte roots, or with want_updates
+        (b200_dstate_overlay_roots_with_updates) one tuple per block shaped as `apply(..., want_updates=True)` returns, entry
+        indices local to the block."""
         args = block_batch_arrays(blocks)
         n = len(blocks)
         roots = np.zeros((max(n, 1), 32), np.uint8)
         s = Stats()
-        self.engine._check(self.engine.lib.b200_dstate_overlay_roots(self.handle, n, *(_ptr(a) for a in args), _ptr(roots), C.byref(s)))
-        return [roots[b].tobytes() for b in range(n)]
+        lib = self.engine.lib
+        if not want_updates:
+            self.engine._check(lib.b200_dstate_overlay_roots(self.handle, n, *(_ptr(a) for a in args), _ptr(roots), C.byref(s)))
+            return [roots[b].tobytes() for b in range(n)]
+        block_acct = args[3]
+        m = int(block_acct[n])
+        au, ar, su, sr = Updates(), Updates(), Updates(), Updates()
+        deleted = np.zeros(max(m, 1), np.uint8)
+        self.engine._check(lib.b200_dstate_overlay_roots_with_updates(
+            self.handle, n, *(_ptr(a) for a in args), _ptr(roots), C.byref(au), C.byref(ar), C.byref(su), C.byref(sr),
+            _ptr(deleted), C.byref(s)))
+        au, ar, su, sr = (updates_to_records(u, lib) for u in (au, ar, su, sr))
+        out = []
+        for b in range(n):
+            lo, hi = int(block_acct[b]), int(block_acct[b + 1])
+            out.append((roots[b].tobytes(), [(0,) + r[1:] for r in au if r[0] == b], [r[1] for r in ar if r[0] == b],
+                        [(r[0] - lo,) + r[1:] for r in su if lo <= r[0] < hi], [(r[0] - lo, r[1]) for r in sr if lo <= r[0] < hi],
+                        deleted[lo:hi].copy()))
+        return out
 
     def account_proofs(self, acct_keys) -> list:
         """-> for every target hashed address the list of node RLPs from the root down (Proof::account_proof)."""

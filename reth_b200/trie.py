@@ -420,6 +420,22 @@ def apply_layout(post, destroyed_slots: bool):
     return touched, (keys, accts, flags, skeys, svals, np.array(offs, np.uint64))
 
 
+def _trie_updates(touched, au, ar, su, sr, deleted) -> TrieUpdates:
+    """TrieUpdates of one block from the records of `DynamicState.apply(..., want_updates=True)` (or of an overlay), entry i
+    being the account touched[i]."""
+    upd = TrieUpdates()
+    upd.account_nodes = _records_to_nodes(au).get(0, {})
+    upd.removed_nodes = {bytes(p) for p in ar}
+    per_entry = _records_to_nodes(su)
+    removed_per_entry: Dict[int, set] = {}
+    for entry, p in sr:
+        removed_per_entry.setdefault(entry, set()).add(bytes(p))
+    for i, k in enumerate(touched):
+        st = StorageTrieUpdates(bool(deleted[i]), per_entry.get(i, {}), removed_per_entry.get(i, set()))
+        upd.insert_storage_updates(k, st)
+    return upd
+
+
 class DynamicStateRoot:
     """Live-path commitment with the WHOLE hashed state resident in HBM (b200_dstate_*): accounts and every storage trie.
 
@@ -448,20 +464,10 @@ class DynamicStateRoot:
         """post: HashedPostState -> (root, TrieUpdates of the block)."""
         touched, block = self._block(post, destroyed_slots=False)
         try:
-            root, au, ar, su, sr, deleted = self.ds.apply(*block, want_updates=True)
+            res = self.ds.apply(*block, want_updates=True)
         except Exception as e:  # noqa: BLE001
             raise StateRootError(str(e)) from e
-        upd = TrieUpdates()
-        upd.account_nodes = _records_to_nodes(au).get(0, {})
-        upd.removed_nodes = {bytes(p) for p in ar}
-        per_entry = _records_to_nodes(su)
-        removed_per_entry: Dict[int, set] = {}
-        for entry, p in sr:
-            removed_per_entry.setdefault(entry, set()).add(bytes(p))
-        for i, k in enumerate(touched):
-            st = StorageTrieUpdates(bool(deleted[i]), per_entry.get(i, {}), removed_per_entry.get(i, set()))
-            upd.insert_storage_updates(k, st)
-        return root, upd
+        return res[0], _trie_updates(touched, *res[1:])
 
     def witness(self, post, mode: str = "legacy", always_include_root_node: bool = False) -> Dict[bytes, bytes]:
         """TrieWitness::compute(post) against the state as it is (crates/trie/trie/src/witness.rs): {keccak(node): node RLP}
@@ -490,18 +496,35 @@ class DynamicStateRoot:
         return, with the state left as it is — to validate a payload, or to finish every payload built on this parent, before
         `commit` keeps one of them.  The posts are siblings on the current state, not a chain.  A chain of uncommitted blocks
         is one post merged with HashedPostState.extend, as MemoryOverlayStateProvider merges its in-memory blocks
-        (crates/chain-state/src/memory_overlay.rs).  No TrieUpdates: `commit` returns those of the block that is kept."""
-        blocks = [self._block(post, destroyed_slots=False)[1] for post in posts]
-        try:
-            return self.ds.overlay_roots(blocks)
-        except ValueError:
-            raise
-        except Exception as e:  # noqa: BLE001
-            raise StateRootError(str(e)) from e
+        (crates/chain-state/src/memory_overlay.rs).  `overlay_roots_with_updates` also returns each block's TrieUpdates."""
+        return self._overlay(posts, False)
 
     def overlay_root(self, post) -> bytes:
         """overlay_roots for one post: the root `commit(post)` would return, without changing the state."""
         return self.overlay_roots([post])[0]
+
+    def overlay_roots_with_updates(self, posts) -> List[Tuple[bytes, TrieUpdates]]:
+        """StateRoot::overlay_root_with_updates (crates/trie/db/src/state.rs:219-230) for a batch of candidate blocks, in one
+        device call (b200_dstate_overlay_roots_with_updates): for each post, (root, TrieUpdates) that describe the same trie
+        tables after the block as `commit(post)`'s, with the state left as it is — what payload validation, BlockBuilder::finish
+        and debug_stateRootWithUpdates keep with a block until it is persisted."""
+        return self._overlay(posts, True)
+
+    def overlay_root_with_updates(self, post) -> Tuple[bytes, TrieUpdates]:
+        """overlay_roots_with_updates for one post."""
+        return self.overlay_roots_with_updates([post])[0]
+
+    def _overlay(self, posts, want_updates: bool):
+        layouts = [self._block(post, destroyed_slots=False) for post in posts]
+        try:
+            res = self.ds.overlay_roots([block for _, block in layouts], want_updates=want_updates)
+        except ValueError:
+            raise
+        except Exception as e:  # noqa: BLE001
+            raise StateRootError(str(e)) from e
+        if not want_updates:
+            return res
+        return [(r[0], _trie_updates(touched, *r[1:])) for (touched, _), r in zip(layouts, res)]
 
     def close(self):
         self.ds.close()

@@ -13,7 +13,14 @@ applies a new block); the first apply is the first sibling, and its root must eq
 root must equal its witness_roots root on the unchanged state.  CUDA-event time on the call's stream and host-call time
 of the C ABI call alone (inputs packed beforehand), after warm-ups, median / min / max over --reps.  Counts per call:
 kernel launches (b200_launch_count), device-to-host read-backs and host-to-device copies from a separate torch.profiler
-run of one call.  Reads the card's name, power limit and SM clock in the same run.  Prints one JSON line."""
+run of one call.  Reads the card's name, power limit and SM clock in the same run.  Prints one JSON line.
+
+    python tools/overlay_bench.py --updates
+
+--updates measures the TrieUpdates instead (b200_dstate_overlay_roots_with_updates): the root-only overlay of the first block
+and of all siblings, each alternating rep by rep with the with-updates call of the same blocks, then b200_dstate_apply with
+updates over a chain of fresh blocks of the same shape.  Each with its time, launches, read-backs and record count
+(updated + removed records of both tries)."""
 import argparse
 import ctypes as C
 import json
@@ -39,11 +46,12 @@ def main():
     ap.add_argument("--siblings", type=int, default=16)
     ap.add_argument("--reps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--updates", action="store_true", help="measure the overlay with TrieUpdates (see above)")
     args = ap.parse_args()
     import torch
 
     from reth_b200 import DynamicState, Engine
-    from reth_b200._lib import Stats, Witness
+    from reth_b200._lib import Stats, Updates, Witness
     from reth_b200.engine import _ptr, block_batch_arrays, witness_batch_arrays
     out = {"card": card()}
     eng = Engine(0)
@@ -89,6 +97,94 @@ def main():
         names = [e.name for e in prof.events()]
         return {"device_ms": spread(dev), "host_call_ms": spread(host), "launches": launches,
                 "readbacks_dtoh": sum(1 for n in names if "DtoH" in n), "copies_htod": sum(1 for n in names if "HtoD" in n)}
+
+    def counts(call):
+        """launches, then device-to-host read-backs and host-to-device copies from a torch.profiler run of one call"""
+        l0 = eng.launch_count()
+        call()
+        launches = eng.launch_count() - l0
+        from torch.profiler import ProfilerActivity, profile
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            call()
+            torch.cuda.synchronize()
+        names = [e.name for e in prof.events()]
+        return {"launches": launches, "readbacks_dtoh": sum(1 for n in names if "DtoH" in n),
+                "copies_htod": sum(1 for n in names if "HtoD" in n)}
+
+    def alternating(calls):
+        """{name: call}: warmed up, then timed rep by rep in turn, so that both see the same machine"""
+        res = {k: counts(c) for k, c in calls.items()}
+        for _ in range(args.warmup):
+            for c in calls.values():
+                c()
+        dev, host = {k: [] for k in calls}, {k: [] for k in calls}
+        for _ in range(args.reps):
+            for k, c in calls.items():
+                torch.cuda.synchronize()
+                ev0.record(stream)
+                t0 = time.perf_counter()
+                c()
+                host[k].append((time.perf_counter() - t0) * 1e3)
+                ev1.record(stream)
+                ev1.synchronize()
+                dev[k].append(ev0.elapsed_time(ev1))
+        for k in calls:
+            res[k].update({"device_ms": spread(dev[k]), "host_call_ms": spread(host[k])})
+        return res
+
+    if args.updates:
+        def overlay_calls(nb):
+            packed = block_batch_arrays(arrays[:nb])
+            roots = np.zeros((nb, 32), np.uint8)
+            deleted = np.zeros(max(len(packed[0]), 1), np.uint8)
+            recs = {}
+
+            def root_only():
+                eng._check(eng.lib.b200_dstate_overlay_roots(ds.handle, nb, *(_ptr(x) for x in packed), _ptr(roots), C.byref(Stats())))
+
+            def with_updates():
+                us = [Updates() for _ in range(4)]
+                eng._check(eng.lib.b200_dstate_overlay_roots_with_updates(ds.handle, nb, *(_ptr(x) for x in packed), _ptr(roots),
+                                                                          *(C.byref(u) for u in us), _ptr(deleted), C.byref(Stats())))
+                recs["records"] = [int(u.n_nodes) for u in us]
+                for u in us:
+                    eng.lib.b200_updates_release(C.byref(u))
+            r = alternating({"root_only": root_only, "with_updates": with_updates})
+            r["with_updates"]["records"] = dict(zip(["acct_updated", "acct_removed", "storage_updated", "storage_removed"],
+                                                    recs["records"]))
+            r["with_updates"]["records"]["total"] = sum(recs["records"])
+            r["blocks"] = nb
+            return r
+        out["overlay_one"] = overlay_calls(1)
+        out["overlay_batch"] = overlay_calls(args.siblings)
+        assert ds.root() == parent
+        chain = iter(block_arrays(make_block(rng, keys, skeys, offs, args.touch, args.slot_writes))
+                     for _ in range(args.warmup + args.reps + 4))
+        cur, recs = {}, {}
+        root = np.zeros(32, np.uint8)
+
+        def apply_updates():
+            a = cur["a"]
+            us = [Updates() for _ in range(4)]
+            deleted = np.zeros(max(len(a[0]), 1), np.uint8)
+            eng._check(eng.lib.b200_dstate_apply(ds.handle, _ptr(a[0]), _ptr(a[1]), _ptr(a[2]), len(a[0]), _ptr(a[3]), _ptr(a[4]),
+                                                 _ptr(a[5]), _ptr(root), *(C.byref(u) for u in us), _ptr(deleted), C.byref(Stats())))
+            recs["records"] = sum(int(u.n_nodes) for u in us)
+            for u in us:
+                eng.lib.b200_updates_release(C.byref(u))
+        out["apply_with_updates_chain"] = measure(apply_updates, before=lambda: cur.__setitem__("a", next(chain)))
+        out["apply_with_updates_chain"]["records"] = recs["records"]
+        out["apply_with_updates_chain"]["note"] = "every rep applies a fresh block of the same shape on top of the previous one"
+        o1 = out["overlay_one"]["with_updates"]["device_ms"]["median"]
+        out["ratios"] = {"updates_over_root_only_one": round(o1 / out["overlay_one"]["root_only"]["device_ms"]["median"], 2),
+                         "updates_over_root_only_batch": round(out["overlay_batch"]["with_updates"]["device_ms"]["median"] /
+                                                               out["overlay_batch"]["root_only"]["device_ms"]["median"], 2),
+                         "overlay_updates_over_apply_updates": round(o1 / out["apply_with_updates_chain"]["device_ms"]["median"], 2)}
+        out["card_after"] = card()
+        print(json.dumps(out))
+        ds.close()
+        eng.close()
+        return
 
     # ---- overlay: one block, then every sibling in one call
     def overlay_case(nb):
