@@ -665,6 +665,32 @@ B200_API int32_t b200_dstate_overlay_roots_with_updates(b200_dstate *, uint64_t 
                                                         uint8_t *roots32, b200_updates *opt_acct_updated, b200_updates *opt_acct_removed,
                                                         b200_updates *opt_storage_updated, b200_updates *opt_storage_removed,
                                                         uint8_t *opt_storage_deleted /* [M] */, b200_stats *opt_stats);
+/* Merkle proofs of the state after one candidate block, against the state as it is, which does not change (reth:
+ * Proof::overlay_multiproof, crates/trie/db/src/proof.rs, which StateProofProvider::multiproof / proof of a
+ * MemoryOverlayStateProvider reach with the in-memory blocks prepended to the input — eth_getProof at a block that is not
+ * persisted, and the proof workers of the state-root task over an OverlayStateProviderFactory).  A chain of in-memory blocks
+ * is one block whose entries are merged, as for b200_dstate_overlay_roots.
+ *   the block   : m account entries in the layout of b200_dstate_apply and with its rules (flags bit 0/1/2, zero value
+ *                 deletes, seg_offsets [m+1]; keys strictly ascending).
+ *   the targets : the layout of b200_dstate_multiproof: n_targets account keys, target i with the slot keys
+ *                 target_slot_offsets[i] .. [i+1] of target_slot_keys32; account keys strictly ascending, and the slot keys
+ *                 of each target (B200_ERR_UNSORTED).
+ * Every output is byte for byte what b200_dstate_apply(block) followed by b200_dstate_multiproof(targets) gives on a twin
+ * state: root32 (nullable) the apply's root; every target's nodes in account_proofs / storage_proofs with the same RLPs, in
+ * the same order, with the same node_depth and node_masks; storage_roots32[i] the storage root of target i after the block
+ * (EMPTY_ROOT_HASH when the account does not exist after it, and each of its slot targets then proves with the single node
+ * 0x80).  m = 0 gives b200_dstate_multiproof of the targets.  Call-level errors are those of b200_dstate_overlay_roots plus
+ * those of b200_dstate_multiproof: B200_ERR_INVALID_ARG for null pointers, offsets that do not start at 0 or are not monotone,
+ * 2^24 or more account targets or slot targets, 2^31-1 or more entries plus revealed items, and a sharded state.  On error
+ * both b200_proofs are released and zeroed.  opt_stats covers the whole call. */
+B200_API int32_t b200_dstate_overlay_multiproof(b200_dstate *, const uint8_t *acct_keys32, const b200_account *accts,
+                                                const uint8_t *acct_flags /* nullable */, uint64_t m, const uint8_t *slot_keys32,
+                                                const uint8_t *values32_be, const uint64_t *seg_offsets /* [m+1] */,
+                                                const uint8_t *target_keys32, uint64_t n_targets,
+                                                const uint64_t *target_slot_offsets /* [n_targets+1] */, const uint8_t *target_slot_keys32,
+                                                uint8_t root32[32] /* nullable */, b200_proofs *account_proofs,
+                                                uint8_t *storage_roots32 /* [n_targets][32] */, b200_proofs *storage_proofs,
+                                                b200_stats *opt_stats);
 /* b200_dstate_apply with the block already in device memory (every input pointer and d_root32 are device pointers;
  * n_entries = d_seg_offsets[m]); the update records, if wanted, still arrive in host memory. */
 B200_API int32_t b200_dstate_apply_dev(b200_dstate *, const void *d_acct_keys32, const void *d_accts, const void *d_acct_flags,

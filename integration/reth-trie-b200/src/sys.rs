@@ -192,6 +192,13 @@ unsafe extern "C" {
                                   slot_keys32: *const u8, account_proofs: *mut b200_proofs, storage_roots32: *mut u8,
                                   storage_proofs: *mut b200_proofs) -> i32;
     pub fn b200_proofs_release(p: *mut b200_proofs);
+    /// multiproof of the state after one candidate block (layout of b200_dstate_apply), the state unchanged
+    pub fn b200_dstate_overlay_multiproof(state: *mut b200_dstate, acct_keys32: *const u8, accts: *const b200_account,
+                                          acct_flags: *const u8, m: u64, slot_keys32: *const u8, values32_be: *const u8,
+                                          seg_offsets: *const u64, target_keys32: *const u8, n_targets: u64,
+                                          target_slot_offsets: *const u64, target_slot_keys32: *const u8, root32: *mut u8,
+                                          account_proofs: *mut b200_proofs, storage_roots32: *mut u8,
+                                          storage_proofs: *mut b200_proofs, opt_stats: *mut b200_stats) -> i32;
     /// CPUs + preferred memory of the calling thread on the GPU's NUMA node (before allocating staging buffers)
     pub fn b200_numa_bind_thread(device_ordinal: i32) -> i32;
 }

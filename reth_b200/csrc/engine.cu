@@ -383,4 +383,5 @@ extern "C" B200_API uint64_t b200_launch_count(const b200_ctx *c) { return c ? c
 #include "eng_items.inl"
 #include "eng_stateless.inl"
 #include "eng_overlay.inl"
+#include "eng_overlay_proofs.inl"
 #include "eng_comm.inl"

@@ -137,15 +137,15 @@ cudaError_t launch_dt_frontier(const DTrieDev &t, const uint8_t *bucket_roots, F
     dt_frontier_kernel<<<1, 512, 0, st>>>(t, bucket_roots, out);
     return cudaGetLastError();
 }
-cudaError_t launch_dt_proof_sizes(const DTrieDev &t, const uint32_t *trie_of_target, const uint8_t *keys, uint64_t n,
+cudaError_t launch_dt_proof_sizes(const DTrieDev &t, const DTrieDev &alt, const uint32_t *trie_of_target, const uint8_t *keys, uint64_t n,
                                   uint32_t *node_count, uint64_t *byte_count, cudaStream_t st) {
-    if (n) dt_proof_size_kernel<<<blocks_for(n, 64), 64, 0, st>>>(t, trie_of_target, keys, n, node_count, byte_count);
+    if (n) dt_proof_size_kernel<<<blocks_for(n, 64), 64, 0, st>>>(t, alt, trie_of_target, keys, n, node_count, byte_count);
     return cudaGetLastError();
 }
-cudaError_t launch_dt_proof_write(const DTrieDev &t, const uint32_t *trie_of_target, const uint8_t *keys, uint64_t n,
+cudaError_t launch_dt_proof_write(const DTrieDev &t, const DTrieDev &alt, const uint32_t *trie_of_target, const uint8_t *keys, uint64_t n,
                                   const uint64_t *node_base, const uint64_t *byte_base, uint8_t *rlp, uint64_t *rlp_offset,
                                   uint8_t *node_depth, uint32_t *node_masks, cudaStream_t st) {
-    if (n) dt_proof_write_kernel<<<blocks_for(n, 64), 64, 0, st>>>(t, trie_of_target, keys, n, node_base, byte_base, rlp, rlp_offset, node_depth,
+    if (n) dt_proof_write_kernel<<<blocks_for(n, 64), 64, 0, st>>>(t, alt, trie_of_target, keys, n, node_base, byte_base, rlp, rlp_offset, node_depth,
                                                                   node_masks);
     return cudaGetLastError();
 }

@@ -14,6 +14,12 @@
 // holds it (reth's CursorSubNode::tree_flag: the branch is stored), so that the fold rebuilds the stored records of the
 // branches on the keys' paths; and every stored branch the reveal queues (not at the empty path) is a removed-node
 // candidate, dropped later when the fold stores a record at the same path.
+//
+// With proof targets (b200_dstate_overlay_multiproof, one block) a queued branch also carries the range of its trie's sorted
+// targets that pass through it: the account targets, or the slot targets of the account target whose key is the entry's.
+// A branch is queued when either range is non-empty.  Targets are not entries: the merge, the rows and the folds do not
+// change.  Afterwards the fold builds every node of the post-block trie on a target's path; the only hash item a target
+// can reach is a branch below an extension that the target leaves.
 
 // nibbles [from, to) of `key` against those of `path`: -1 / 0 / 1
 __device__ __forceinline__ int ov_cmp_nibbles(const uint8_t *key, const uint8_t *path, uint32_t from, uint32_t to) {
@@ -79,14 +85,15 @@ __device__ __forceinline__ SlItem &ov_item(SlItem *items, uint32_t *n_items, uin
     return it;
 }
 
-// Child word w of a branch at depth pd (-1: w is the root word of its trie) with the targets [lo, hi) that pass through
-// the child's slot, and the parent's tree-mask bit for that slot (`tree`; for a root word ov_root_tree): a leaf is an
-// item; a branch is queued with the targets that share its whole path, or, when none do and its RLP is at least 32 bytes,
+// Child word w of a branch at depth pd (-1: w is the root word of its trie) with the entries [lo, hi) and the proof targets
+// [tlo, thi) that pass through the child's slot, and the parent's tree-mask bit for that slot (`tree`; for a root word ov_root_tree): a leaf is an
+// item; a branch is queued with the keys that share its whole path, or, when none do and its RLP is at least 32 bytes,
 // is an item holding the hash of the branch itself (under an implicit extension the reference its parent holds is the
 // extension's, so the branch is re-hashed).  A branch shorter than 32 bytes has no hash form: it is queued with its
 // (possibly empty) range and its children become items.
 __device__ void ov_word(const DTrieDev &t, const StatelessDev &s, uint32_t w, int pd, uint32_t tree, uint32_t trie, uint32_t block,
-                        uint32_t lo, uint32_t hi, OvNode *next, uint32_t *n_next, SlItem *items, uint32_t *n_items, uint8_t *vals) {
+                        uint32_t lo, uint32_t hi, uint32_t tlo, uint32_t thi, OvNode *next, uint32_t *n_next, SlItem *items,
+                        uint32_t *n_items, uint8_t *vals) {
     uint32_t idx;
     if (w & DT_LEAF) {
         const uint32_t x = w & ~DT_LEAF;
@@ -100,20 +107,27 @@ __device__ void ov_word(const DTrieDev &t, const StatelessDev &s, uint32_t w, in
     const uint32_t d = t.ndepth[w];
     const uint8_t *nk = t.nkey + 32 * (uint64_t)w;
     const bool ext = (int)d > pd + 1;
-    if (ext && lo < hi) {  // the targets that diverge inside the extension do not reach the branch
+    if (ext && lo < hi) {  // the keys that diverge inside the extension do not reach the branch
         const uint8_t *keys = trie >= s.m ? s.akeys : s.skeys;
         lo = ov_first_above(keys, lo, hi, nk, (uint32_t)(pd + 1), d, -1);
         hi = ov_first_above(keys, lo, hi, nk, (uint32_t)(pd + 1), d, 0);
     }
+    if (ext && tlo < thi) {
+        const uint8_t *keys = trie >= s.m ? s.tkeys : s.tskeys;
+        tlo = ov_first_above(keys, tlo, thi, nk, (uint32_t)(pd + 1), d, -1);
+        thi = ov_first_above(keys, tlo, thi, nk, (uint32_t)(pd + 1), d, 0);
+    }
     uint32_t sm, tm, hm;
     const uint32_t payload = dt_branch_payload<false>(t, w, sm, tm, hm), blen = list_header_len(payload) + payload;
-    if (lo < hi || blen < 32) {
+    if (lo < hi || tlo < thi || blen < 32) {
         OvNode &e = next[atomicAdd(n_next, 1u)];
         e.node = w;
         e.trie = trie;
         e.block = block;
         e.lo = lo;
         e.hi = hi;
+        e.tlo = tlo;
+        e.thi = thi;
         return;
     }
     SlItem &it = ov_item(items, n_items, trie, block, idx);
@@ -152,7 +166,9 @@ __global__ void ov_seed_kernel(DTrieDev ta, DTrieDev ts, StatelessDev s, const u
     if (i < s.n_blocks) {
         for (int k = 0; k < 32; k++) parent[32 * i + k] = root[k];
         const uint32_t lo = (uint32_t)s.block_acct[i], hi = (uint32_t)s.block_acct[i + 1], w = ta.troot[0];
-        if (lo < hi && w != DT_NONE) ov_word(ta, s, w, -1, ov_root_tree(ta, w), (uint32_t)(s.m + i), (uint32_t)i, lo, hi, q, n_q, items, n_items, vals);
+        if (lo < hi && w != DT_NONE)
+            ov_word(ta, s, w, -1, ov_root_tree(ta, w), (uint32_t)(s.m + i), (uint32_t)i, lo, hi, 0, (uint32_t)s.n_t, q, n_q, items, n_items,
+                    vals);
         return;
     }
     const uint64_t a = i - s.n_blocks;
@@ -164,12 +180,27 @@ __global__ void ov_seed_kernel(DTrieDev ta, DTrieDev ts, StatelessDev s, const u
     if (found) found[a] = loc.found ? 1 : 0;
     if (!reveal || !loc.found) return;
     const uint32_t w = ts.troot[loc.child & ~DT_LEAF];
-    if (w != DT_NONE)
-        ov_word(ts, s, w, -1, ov_root_tree(ts, w), (uint32_t)a, sl_block_of_entry(s, a), (uint32_t)s.seg[a], (uint32_t)s.seg[a + 1], q, n_q, items, n_items,
-                vals);
+    if (w == DT_NONE) return;
+    uint32_t tlo = 0, thi = 0;  // the slot targets of the account target with this entry's key
+    if (s.n_t) {
+        const uint8_t *key = s.akeys + 32 * a;
+        uint64_t lo = 0, hi = s.n_t;  // first account target >= key
+        while (lo < hi) {
+            const uint64_t mid = (lo + hi) >> 1;
+            if (ov_cmp_nibbles(s.tkeys + 32 * mid, key, 0, 64) < 0) lo = mid + 1;
+            else hi = mid;
+        }
+        if (lo < s.n_t && ov_cmp_nibbles(s.tkeys + 32 * lo, key, 0, 64) == 0) {
+            tlo = (uint32_t)s.tseg[lo];
+            thi = (uint32_t)s.tseg[lo + 1];
+        }
+    }
+    ov_word(ts, s, w, -1, ov_root_tree(ts, w), (uint32_t)a, sl_block_of_entry(s, a), (uint32_t)s.seg[a], (uint32_t)s.seg[a + 1], tlo, thi, q,
+            n_q, items, n_items, vals);
 }
 
-// One level: every queued branch splits its targets by the nibble at its depth and hands each child its part; a stored one
+// One level: every queued branch splits its entries and its targets by the nibble at its depth and hands each child its
+// parts; a stored one
 // (not at the empty path) is a removed-node candidate when rm keeps them.
 __global__ void ov_reveal_kernel(DTrieDev ta, DTrieDev ts, StatelessDev s, const OvNode *q, uint32_t nq, OvNode *next, uint32_t *n_next,
                                  SlItem *items, uint32_t *n_items, uint8_t *vals, OvRemoved rm) {
@@ -188,16 +219,23 @@ __global__ void ov_reveal_kernel(DTrieDev ta, DTrieDev ts, StatelessDev s, const
         cand[2 * k] = e.trie;
         cand[2 * k + 1] = e.node;
     }
-    uint32_t lo = e.lo;
-    for (uint32_t c = 0; c < 16; c++) {
-        uint32_t hi = lo, top = e.hi;  // first target in [lo, e.hi) whose nibble d is above c
-        while (hi < top) {
-            const uint32_t mid = (hi + top) >> 1;
-            if (sl_nib(keys + 32 * (uint64_t)mid, d) <= c) hi = mid + 1;
+    const uint8_t *tkeys = account ? s.tkeys : s.tskeys;
+    // first key in [lo, top) whose nibble d is above c
+    auto split = [d](const uint8_t *ks, uint32_t lo, uint32_t top, uint32_t c) {
+        while (lo < top) {
+            const uint32_t mid = (lo + top) >> 1;
+            if (sl_nib(ks + 32 * (uint64_t)mid, d) <= c) lo = mid + 1;
             else top = mid;
         }
-        if (ch[c] != DT_NONE) ov_word(t, s, ch[c], (int)d, (tree_mask >> c) & 1u, e.trie, e.block, lo, hi, next, n_next, items, n_items, vals);
+        return lo;
+    };
+    uint32_t lo = e.lo, tlo = e.tlo;
+    for (uint32_t c = 0; c < 16; c++) {
+        const uint32_t hi = split(keys, lo, e.hi, c), thi = tlo < e.thi ? split(tkeys, tlo, e.thi, c) : tlo;
+        if (ch[c] != DT_NONE)
+            ov_word(t, s, ch[c], (int)d, (tree_mask >> c) & 1u, e.trie, e.block, lo, hi, tlo, thi, next, n_next, items, n_items, vals);
         lo = hi;
+        tlo = thi;
     }
 }
 

@@ -48,6 +48,10 @@ static __device__ void dt_keccak_global(const uint8_t *p, uint32_t len, uint32_t
 // branch below a diverging extension is kept too; only nodes whose path is at least `min_len` nibbles long are kept (an
 // extension and its branch by the extension's path: ProofV2Target::with_min_len); WT_ROOT_ONLY stops after the root
 // node (with its branch when it is an extension), WT_FIRST_ONLY after the first node.
+// An arena made from an items fold (b200_dstate_overlay_multiproof) also holds hash leaves (lmeta META_ISNODE): the hash of a
+// branch at path lkey[..lnib) that the fold did not open.  A target reaches one only where it leaves the extension above
+// that branch: the proof ends with the extension node, whose child is the hash.  A target that shares the whole path
+// would need the branch itself, which the fold does not have: a sticky B200_DEVERR_CORRUPT, never a wrong proof.
 template <bool WRITE, bool WITNESS = false>
 static __device__ void dt_proof_walk(const DTrieDev &t, uint32_t trie, const uint8_t *key, uint32_t &n_nodes, uint64_t &n_bytes,
                                      uint8_t *rlp, uint64_t byte_base, uint64_t *rlp_offset, uint8_t *node_depth, uint32_t *node_masks,
@@ -78,9 +82,29 @@ static __device__ void dt_proof_walk(const DTrieDev &t, uint32_t trie, const uin
     for (int hops = 0; hops <= DT_MAX_HOPS; hops++) {
         if (cur & DT_LEAF) {
             const uint32_t x = cur & ~DT_LEAF;
+            const uint8_t *val = t.lval + (uint64_t)t.val_stride * x;
+            if (!WITNESS && (t.lmeta[x] & META_ISNODE)) {
+                const uint8_t *hk = t.lkey + 32 * (uint64_t)x;
+                const uint32_t L = t.lnib[x];
+                if ((int)L <= pd + 1 || dt_lcp(key, hk, (uint32_t)(pd + 1), L) == L) {
+                    atomicExch(t.err, B200_DEVERR_CORRUPT);
+                    return;
+                }
+                uint32_t child[8];
+                for (int w = 0; w < 8; w++)
+                    child[w] = (uint32_t)val[4 * w] | ((uint32_t)val[4 * w + 1] << 8) | ((uint32_t)val[4 * w + 2] << 16) |
+                               ((uint32_t)val[4 * w + 3] << 24);
+                const uint32_t m = L - (uint32_t)(pd + 1), hp_len = 1 + (m >> 1), path_str = hp_len == 1 ? 1 : 1 + hp_len;
+                const uint32_t epayload = path_str + 33, elen = list_header_len(epayload) + epayload;
+                if (WRITE) {
+                    LinBuf lb{rlp + byte_base + n_bytes, 0};
+                    encode_extension(lb, hk, (uint32_t)(pd + 1), L, child, 0u);
+                }
+                begin_node(elen, pd + 1);
+                return;
+            }
             uint32_t k[8];
             load32_nc(t.lkey + 32 * (uint64_t)x, k);
-            const uint8_t *val = t.lval + (uint64_t)t.val_stride * x;
             const uint8_t *sr = t.lsroot ? t.lsroot + 32 * (uint64_t)x : nullptr;
             if (WITNESS && (uint32_t)(pd + 1) < min_len) return;
             CountBuf cb{0};
@@ -152,8 +176,9 @@ static __device__ void dt_proof_walk(const DTrieDev &t, uint32_t trie, const uin
     atomicExch(t.err, B200_DEVERR_CORRUPT);
 }
 
-// trie_of_target: nullptr = trie 0; DT_NONE entries (storage of an absent account) prove against the empty trie
-__global__ void dt_proof_size_kernel(DTrieDev t, const uint32_t *__restrict__ trie_of_target, const uint8_t *__restrict__ keys,
+// trie_of_target: nullptr = trie 0 of t; DT_NONE entries (storage of an absent account) prove against the empty trie;
+// DT_ALT | r: trie r of alt
+__global__ void dt_proof_size_kernel(DTrieDev t, DTrieDev alt, const uint32_t *__restrict__ trie_of_target, const uint8_t *__restrict__ keys,
                                      uint64_t n, uint32_t *__restrict__ node_count, uint64_t *__restrict__ byte_count) {
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
@@ -164,12 +189,12 @@ __global__ void dt_proof_size_kernel(DTrieDev t, const uint32_t *__restrict__ tr
         nn = 1;
         nb = 1;
     } else {
-        dt_proof_walk<false>(t, trie, keys + 32 * i, nn, nb, nullptr, 0, nullptr, nullptr, nullptr, 0);
+        dt_proof_walk<false>(trie & DT_ALT ? alt : t, trie & ~DT_ALT, keys + 32 * i, nn, nb, nullptr, 0, nullptr, nullptr, nullptr, 0);
     }
     node_count[i] = nn;
     byte_count[i] = nb;
 }
-__global__ void dt_proof_write_kernel(DTrieDev t, const uint32_t *__restrict__ trie_of_target, const uint8_t *__restrict__ keys,
+__global__ void dt_proof_write_kernel(DTrieDev t, DTrieDev alt, const uint32_t *__restrict__ trie_of_target, const uint8_t *__restrict__ keys,
                                       uint64_t n, const uint64_t *__restrict__ node_base, const uint64_t *__restrict__ byte_base,
                                       uint8_t *__restrict__ rlp, uint64_t *__restrict__ rlp_offset, uint8_t *__restrict__ node_depth,
                                       uint32_t *__restrict__ node_masks) {
@@ -184,7 +209,8 @@ __global__ void dt_proof_write_kernel(DTrieDev t, const uint32_t *__restrict__ t
         node_depth[node_base[i]] = 0;
         node_masks[node_base[i]] = 0;
     } else {
-        dt_proof_walk<true>(t, trie, keys + 32 * i, nn, nb, rlp, byte_base[i], rlp_offset, node_depth, node_masks, node_base[i]);
+        dt_proof_walk<true>(trie & DT_ALT ? alt : t, trie & ~DT_ALT, keys + 32 * i, nn, nb, rlp, byte_base[i], rlp_offset, node_depth,
+                            node_masks, node_base[i]);
     }
 }
 // the account leaf (= storage trie id) of one account key, DT_NONE when the account does not exist

@@ -200,6 +200,7 @@ enum : int {
 struct DTrieDev {
     // leaves [lcap]
     uint8_t *lkey, *lval, *lsroot, *lref, *lmeta;  // lval: 72-byte account or 32-byte slot value; lsroot: accounts only
+    const uint8_t *lnib;  // arenas made from an items fold only (else null): path length of a hash leaf (lmeta META_ISNODE)
     uint32_t *lparent, *ltrie;                     // ltrie / ntrie: owning trie (nullptr = a single trie, id 0)
     uint8_t *lseed;
     // nodes [ncap]
@@ -262,9 +263,12 @@ cudaError_t launch_dt_expand_tries(const uint64_t *seg_offsets, uint64_t m, cons
 cudaError_t launch_dt_nibble_tries(const uint8_t *keys, uint64_t m, uint32_t *trie_of_key, cudaStream_t st);
 cudaError_t launch_dt_frontier(const DTrieDev &t, const uint8_t *bucket_roots, FrontierEntryDev *out, cudaStream_t st);
 
-cudaError_t launch_dt_proof_sizes(const DTrieDev &t, const uint32_t *trie_of_target, const uint8_t *keys, uint64_t n,
+// Proof targets: trie_of_target[i] = a trie of t, DT_NONE (the empty trie), or DT_ALT | a trie of `alt` (the second arena
+// of a call whose targets prove against two: the resident state and an overlay's fold); nullptr = trie 0 of t.
+constexpr uint32_t DT_ALT = 0x80000000u;
+cudaError_t launch_dt_proof_sizes(const DTrieDev &t, const DTrieDev &alt, const uint32_t *trie_of_target, const uint8_t *keys, uint64_t n,
                                   uint32_t *node_count, uint64_t *byte_count, cudaStream_t st);
-cudaError_t launch_dt_proof_write(const DTrieDev &t, const uint32_t *trie_of_target, const uint8_t *keys, uint64_t n,
+cudaError_t launch_dt_proof_write(const DTrieDev &t, const DTrieDev &alt, const uint32_t *trie_of_target, const uint8_t *keys, uint64_t n,
                                   const uint64_t *node_base, const uint64_t *byte_base, uint8_t *rlp, uint64_t *rlp_offset,
                                   uint8_t *node_depth, uint32_t *node_masks, cudaStream_t st);
 cudaError_t launch_dt_find_leaves(const DTrieDev &t, const uint8_t *keys, uint64_t n, uint32_t *leaf_out, uint8_t *sroot_out, cudaStream_t st);
@@ -335,6 +339,11 @@ struct StatelessDev {
     const uint8_t *skeys, *svals;  // [n_e][32]
     uint64_t n_blocks, m, n_e;
     uint32_t *status;            // [n_blocks] SL_INCOMPLETE | SL_INVALID
+    // overlay multiproof (one block): the proof targets, which the reveal follows as well as the entries
+    const uint8_t *tkeys;        // [n_t][32] account targets, ascending
+    const uint64_t *tseg;        // [n_t + 1] slot targets of account target i
+    const uint8_t *tskeys;       // [tseg[n_t]][32]
+    uint64_t n_t;
 };
 struct SlNode {  // a queued node: trie, path (packed nibbles, zero-padded) and depth, RLP at rlp[off, off + len)
     uint8_t path[32];
@@ -372,8 +381,9 @@ cudaError_t launch_sl_rows(const StatelessDev &s, const SlItem *fin, uint64_t lo
 cudaError_t launch_sl_finish(const StatelessDev &s, const uint8_t *acc_roots, uint8_t *out, cudaStream_t st);
 
 // ------------------------------------------------------------------------------------------------ overlay roots (tk_overlay.cuh)
-struct OvNode {  // a queued branch of an arena: trie id of the call, block, and the targets [lo, hi) that pass through it
-    uint32_t node, trie, block, lo, hi;
+struct OvNode {  // a queued branch of an arena: trie id of the call, block, the entries [lo, hi) and the proof targets [tlo, thi)
+                 // that pass through it
+    uint32_t node, trie, block, lo, hi, tlo, thi;
 };
 constexpr uint32_t OV_STRIDE = 112;  // value bytes of item i at OV_STRIDE * i: rlp(TrieAccount) (<= 110), rlp(U256) (<= 33), a hash
 // Removed-node candidates of an overlay with TrieUpdates: (trie id of the call, arena node) of every stored branch that the

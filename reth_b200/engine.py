@@ -914,12 +914,9 @@ class DynamicState:
                 out[nib[:depth]] = rlp
         return out
 
-    def multiproof(self, targets: dict) -> dict:
-        """Proof::multiproof(MultiProofTargets) in one device call.  targets: {hashed address: iterable of hashed slots}.
-        -> {"account_subtree": {path: rlp}, "branch_node_masks": {path: (hash_mask, tree_mask)},
-            "storages": {address: {"root": bytes, "subtree": {path: rlp}, "branch_node_masks": {...}}}} — the maps of
-        MultiProof / StorageMultiProof (crates/trie/common/src/proofs.rs:180-188,594-602); branch_node_masks holds the
-        branch nodes of the proof that reth stores in its trie tables (what Proof::with_branch_node_masks(true) collects)."""
+    @staticmethod
+    def _multiproof_targets(targets: dict) -> tuple:
+        """MultiProofTargets in the ABI layout: (sorted addresses, account keys, slot offsets, slot keys, slot key list)."""
         addrs = sorted(targets)
         n = len(addrs)
         ak = np.frombuffer(b"".join(addrs), np.uint8).reshape(n, 32) if n else np.zeros((0, 32), np.uint8)
@@ -929,14 +926,15 @@ class DynamicState:
             slots.extend(sl)
             offs.append(len(slots))
         sk = np.frombuffer(b"".join(slots), np.uint8).reshape(len(slots), 32) if slots else np.zeros((0, 32), np.uint8)
-        so = np.array(offs, np.uint64)
-        sroots = np.zeros((max(n, 1), 32), np.uint8)
-        pa, ps = Proofs(), Proofs()
-        self.engine._check(self.engine.lib.b200_dstate_multiproof(self.handle, _ptr(ak), n, _ptr(so), _ptr(sk), C.byref(pa), _ptr(sroots),
-                                                                  C.byref(ps)))
+        return addrs, ak, np.array(offs, np.uint64), sk, slots
+
+    def _multiproof_dict(self, addrs, offs, slots, pa, sroots, ps, with_nodes: bool) -> dict:
+        """The maps of multiproof() from the two b200_proofs (released here); with_nodes adds every target's raw node list
+        [(node_depth, rlp, node_masks)] in order: "account_nodes"[i] and "storage_nodes"[j] (slot j over all accounts)."""
         nib = lambda k: bytes(x for b in k for x in (b >> 4, b & 15))
         out = {"account_subtree": {}, "branch_node_masks": {}, "storages": {}}
-        for key, nodes in zip(addrs, self._take_proofs(pa, with_masks=True)):
+        ap = self._take_proofs(pa, with_masks=True)
+        for key, nodes in zip(addrs, ap):
             kn = nib(key)
             for depth, rlp, masks in nodes:
                 out["account_subtree"][kn[:depth]] = rlp
@@ -945,13 +943,47 @@ class DynamicState:
         sp = self._take_proofs(ps, with_masks=True)
         for i, a in enumerate(addrs):
             sub, bm = {}, {}
-            for j in range(offs[i], offs[i + 1]):
+            for j in range(int(offs[i]), int(offs[i + 1])):
                 kn = nib(slots[j])
                 for depth, rlp, masks in sp[j]:
                     sub[kn[:depth]] = rlp
                     if masks:
                         bm[kn[:depth]] = (masks >> 16, masks & 0xFFFF)
             out["storages"][a] = {"root": sroots[i].tobytes(), "subtree": sub, "branch_node_masks": bm}
+        if with_nodes:
+            out["account_nodes"], out["storage_nodes"] = ap, sp
+        return out
+
+    def multiproof(self, targets: dict, with_nodes: bool = False) -> dict:
+        """Proof::multiproof(MultiProofTargets) in one device call.  targets: {hashed address: iterable of hashed slots}.
+        -> {"account_subtree": {path: rlp}, "branch_node_masks": {path: (hash_mask, tree_mask)},
+            "storages": {address: {"root": bytes, "subtree": {path: rlp}, "branch_node_masks": {...}}}} — the maps of
+        MultiProof / StorageMultiProof (crates/trie/common/src/proofs.rs:180-188,594-602); branch_node_masks holds the
+        branch nodes of the proof that reth stores in its trie tables (what Proof::with_branch_node_masks(true) collects).
+        with_nodes: also every target's node list, in order (see _multiproof_dict)."""
+        addrs, ak, so, sk, slots = self._multiproof_targets(targets)
+        n = len(addrs)
+        sroots = np.zeros((max(n, 1), 32), np.uint8)
+        pa, ps = Proofs(), Proofs()
+        self.engine._check(self.engine.lib.b200_dstate_multiproof(self.handle, _ptr(ak), n, _ptr(so), _ptr(sk), C.byref(pa), _ptr(sroots),
+                                                                  C.byref(ps)))
+        return self._multiproof_dict(addrs, so, slots, pa, sroots, ps, with_nodes)
+
+    def overlay_multiproof(self, block, targets: dict, with_nodes: bool = False) -> dict:
+        """b200_dstate_overlay_multiproof: multiproof(targets) of the state after `block`, against the state as it is (the
+        state does not change; Proof::overlay_multiproof).  block: an `apply` array tuple (acct_keys, accounts, flags,
+        slot_keys, values, seg_offsets).  -> the dict of multiproof() plus "root", the root `apply(*block)` would return."""
+        keys, accts, flags, _, skeys, svals, seg = block_batch_arrays([block])
+        addrs, ak, so, sk, slots = self._multiproof_targets(targets)
+        n = len(addrs)
+        sroots = np.zeros((max(n, 1), 32), np.uint8)
+        root = np.zeros(32, np.uint8)
+        pa, ps, s = Proofs(), Proofs(), Stats()
+        self.engine._check(self.engine.lib.b200_dstate_overlay_multiproof(
+            self.handle, _ptr(keys), _ptr(accts), _ptr(flags), len(keys), _ptr(skeys), _ptr(svals), _ptr(seg), _ptr(ak), n, _ptr(so),
+            _ptr(sk), _ptr(root), C.byref(pa), _ptr(sroots), C.byref(ps), C.byref(s)))
+        out = self._multiproof_dict(addrs, so, slots, pa, sroots, ps, with_nodes)
+        out["root"] = root.tobytes()
         return out
 
     def witness(self, acct_keys, accounts, flags, slot_keys, values, seg_offsets, mode: str = "legacy",

@@ -514,6 +514,21 @@ class DynamicStateRoot:
         """overlay_roots_with_updates for one post."""
         return self.overlay_roots_with_updates([post])[0]
 
+    def overlay_multiproof(self, post, targets) -> dict:
+        """StateProofProvider::multiproof(input, targets) of a MemoryOverlayStateProvider (crates/chain-state/src/
+        memory_overlay.rs; Proof::overlay_multiproof, crates/trie/db/src/proof.rs) in one device call
+        (b200_dstate_overlay_multiproof): the proofs of `targets` ({hashed address: hashed slots}) in the state after `post`,
+        with the state left as it is — eth_getProof at a block that is not persisted, and the proof workers of the state-root
+        task.  A chain of in-memory blocks is one post merged with HashedPostState.extend.  -> the dict of
+        DynamicState.multiproof plus "root", the root `commit(post)` would return."""
+        _, block = self._block(post, destroyed_slots=False)
+        try:
+            return self.ds.overlay_multiproof(block, targets)
+        except ValueError:
+            raise
+        except Exception as e:  # noqa: BLE001
+            raise StateRootError(str(e)) from e
+
     def _overlay(self, posts, want_updates: bool):
         layouts = [self._block(post, destroyed_slots=False) for post in posts]
         try:

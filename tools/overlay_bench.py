@@ -20,7 +20,14 @@ run of one call.  Reads the card's name, power limit and SM clock in the same ru
 --updates measures the TrieUpdates instead (b200_dstate_overlay_roots_with_updates): the root-only overlay of the first block
 and of all siblings, each alternating rep by rep with the with-updates call of the same blocks, then b200_dstate_apply with
 updates over a chain of fresh blocks of the same shape.  Each with its time, launches, read-backs and record count
-(updated + removed records of both tries)."""
+(updated + removed records of both tries).
+
+    python tools/overlay_bench.py --proofs
+
+--proofs measures the overlay multiproof (b200_dstate_overlay_multiproof) of the first block, alternating rep by rep: with
+the block's accounts and their written slots as targets (what the proof workers ask for); with --touch untouched accounts
+as targets; b200_dstate_multiproof of those untouched targets on the resident state; and b200_dstate_overlay_roots of the
+block.  Each with its time, launches, read-backs and proof node count (account + storage proofs)."""
 import argparse
 import ctypes as C
 import json
@@ -47,11 +54,12 @@ def main():
     ap.add_argument("--reps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--updates", action="store_true", help="measure the overlay with TrieUpdates (see above)")
+    ap.add_argument("--proofs", action="store_true", help="measure the overlay multiproof (see above)")
     args = ap.parse_args()
     import torch
 
     from reth_b200 import DynamicState, Engine
-    from reth_b200._lib import Stats, Updates, Witness
+    from reth_b200._lib import Proofs, Stats, Updates, Witness
     from reth_b200.engine import _ptr, block_batch_arrays, witness_batch_arrays
     out = {"card": card()}
     eng = Engine(0)
@@ -131,6 +139,65 @@ def main():
         for k in calls:
             res[k].update({"device_ms": spread(dev[k]), "host_call_ms": spread(host[k])})
         return res
+
+    if args.proofs:
+        a0 = arrays[0]
+        m = len(a0[0])
+        block_keys = {a0[0][i].tobytes() for i in range(m)}
+        # the block's accounts with their written slots; untouched resident accounts (no slot targets)
+        written = (a0[0], np.asarray(a0[5], np.uint64), a0[3])
+        picks = np.sort(rng.choice(len(keys), 2 * args.touch, replace=False))
+        untouched = np.ascontiguousarray(np.stack([keys[i] for i in picks if keys[i].tobytes() not in block_keys][:args.touch]))
+        plain = (untouched, np.zeros(len(untouched) + 1, np.uint64), np.zeros((0, 32), np.uint8))
+        root = np.zeros(32, np.uint8)
+        roots = np.zeros((1, 32), np.uint8)
+        nodes = {}
+
+        def take(name, pa, ps):
+            nodes[name] = int(pa.n_nodes) + int(ps.n_nodes)
+            eng.lib.b200_proofs_release(C.byref(pa))
+            eng.lib.b200_proofs_release(C.byref(ps))
+
+        def overlay_proof(name, tg):
+            tk, to, ts = tg
+            sroots = np.zeros((max(len(tk), 1), 32), np.uint8)
+
+            def call():
+                pa, ps = Proofs(), Proofs()
+                eng._check(eng.lib.b200_dstate_overlay_multiproof(
+                    ds.handle, *(_ptr(x) for x in a0[:3]), m, *(_ptr(x) for x in a0[3:]), _ptr(tk), len(tk), _ptr(to), _ptr(ts),
+                    _ptr(root), C.byref(pa), _ptr(sroots), C.byref(ps), C.byref(Stats())))
+                take(name, pa, ps)
+            return call
+
+        def resident_proof():
+            pa, ps = Proofs(), Proofs()
+            sroots = np.zeros((len(untouched), 32), np.uint8)
+            eng._check(eng.lib.b200_dstate_multiproof(ds.handle, _ptr(plain[0]), len(plain[0]), _ptr(plain[1]), _ptr(plain[2]),
+                                                      C.byref(pa), _ptr(sroots), C.byref(ps)))
+            take("resident_multiproof_untouched", pa, ps)
+
+        packed = block_batch_arrays(arrays[:1])
+
+        def overlay_root():
+            eng._check(eng.lib.b200_dstate_overlay_roots(ds.handle, 1, *(_ptr(x) for x in packed), _ptr(roots), C.byref(Stats())))
+        calls = {"overlay_multiproof_block_targets": overlay_proof("overlay_multiproof_block_targets", written),
+                 "overlay_multiproof_untouched": overlay_proof("overlay_multiproof_untouched", plain),
+                 "resident_multiproof_untouched": resident_proof, "overlay_roots": overlay_root}
+        res = alternating(calls)
+        for k in res:
+            res[k]["proof_nodes"] = nodes.get(k)
+        out.update(res)
+        out["targets"] = {"block_accounts": m, "block_written_slots": int(len(a0[3])), "untouched_accounts": len(untouched)}
+        assert root.tobytes() == roots[0].tobytes() and ds.root() == parent
+        mo = out["overlay_roots"]["device_ms"]["median"]
+        out["ratios"] = {k + "_over_overlay_roots": round(out[k]["device_ms"]["median"] / mo, 2)
+                         for k in ("overlay_multiproof_block_targets", "overlay_multiproof_untouched", "resident_multiproof_untouched")}
+        out["card_after"] = card()
+        print(json.dumps(out))
+        ds.close()
+        eng.close()
+        return
 
     if args.updates:
         def overlay_calls(nb):
