@@ -691,6 +691,32 @@ B200_API int32_t b200_dstate_overlay_multiproof(b200_dstate *, const uint8_t *ac
                                                 uint8_t root32[32] /* nullable */, b200_proofs *account_proofs,
                                                 uint8_t *storage_roots32 /* [n_targets][32] */, b200_proofs *storage_proofs,
                                                 b200_stats *opt_stats);
+/* Execution witness of a block whose parent is a candidate block on top of the state as it is, which does not change
+ * (reth: StateProofProvider::witness(input, target, mode) of a MemoryOverlayStateProvider — debug_executionWitness and the
+ * invalid-block witness hook when the parent block is not persisted).  A chain of in-memory blocks is one overlay block whose
+ * entries are merged, as for b200_dstate_overlay_roots.  Both blocks come in the layout of b200_dstate_apply and with its
+ * rules; the target block exactly as b200_dstate_witness takes it.
+ * out is byte for byte the map that b200_dstate_apply(overlay) followed by b200_dstate_witness(target, mode,
+ * always_include_root) gives on a twin state, and overlay_root32 (nullable) that apply's root: the parent root a stateless
+ * client checks the witness against.  Hence:
+ *   - ov_m = 0 gives b200_dstate_witness of the target (overlay_root32: the current root);
+ *   - m = 0 gives the empty map, or with always_include_root { overlay root: its root node } ({ EMPTY_ROOT_HASH: 0x80 } when
+ *     the overlay empties the state);
+ *   - both modes as b200_dstate_witness, the removal rule of a live account entry judged on the account after the overlay.
+ * Call-level errors are those of b200_dstate_witness and b200_dstate_overlay_roots: B200_ERR_INVALID_ARG for null pointers,
+ * offsets that do not start at 0 or are not monotone, a bad mode, 2^24 or more target entries or slots, 2^31-1 or more
+ * entries plus revealed items, and a sharded state; B200_ERR_UNSORTED for keys not strictly ascending in either block.  On
+ * error out is released and zeroed.  opt_stats covers the whole call. */
+B200_API int32_t b200_dstate_overlay_witness(
+    b200_dstate *,
+    /* the overlay: in-memory blocks merged, b200_dstate_apply layout and rules */
+    const uint8_t *ov_acct_keys32, const b200_account *ov_accts, const uint8_t *ov_acct_flags /* nullable */, uint64_t ov_m,
+    const uint8_t *ov_slot_keys32, const uint8_t *ov_values32_be, const uint64_t *ov_seg_offsets /* [ov_m+1] */,
+    /* the target block: the same layout, exactly what b200_dstate_witness takes */
+    const uint8_t *acct_keys32, const b200_account *accts, const uint8_t *acct_flags /* nullable */, uint64_t m,
+    const uint8_t *slot_keys32, const uint8_t *values32_be, const uint64_t *seg_offsets /* [m+1] */,
+    int32_t mode, int32_t always_include_root,
+    uint8_t overlay_root32[32] /* nullable */, b200_witness *out, b200_stats *opt_stats);
 /* b200_dstate_apply with the block already in device memory (every input pointer and d_root32 are device pointers;
  * n_entries = d_seg_offsets[m]); the update records, if wanted, still arrive in host memory. */
 B200_API int32_t b200_dstate_apply_dev(b200_dstate *, const void *d_acct_keys32, const void *d_accts, const void *d_acct_flags,

@@ -94,6 +94,12 @@ pub struct b200_proofs {
     pub n_targets: u64, pub node_offset: *mut u64, pub n_nodes: u64, pub rlp_offset: *mut u64, pub rlp: *mut u8,
     pub node_depth: *mut u8, pub node_masks: *mut u32, pub _owner: *mut c_void,
 }
+#[repr(C)]
+pub struct b200_witness {
+    pub n: u64, pub hashes32: *mut u8, pub rlp_offset: *mut u64, pub rlp: *mut u8, pub _owner: *mut c_void,
+}
+pub const B200_WITNESS_LEGACY: i32 = 0;
+pub const B200_WITNESS_CANONICAL: i32 = 1;
 pub const B200_COMM_ID_BYTES: usize = 128;
 
 pub const B200_OK: i32 = 0;
@@ -199,6 +205,15 @@ unsafe extern "C" {
                                           target_slot_offsets: *const u64, target_slot_keys32: *const u8, root32: *mut u8,
                                           account_proofs: *mut b200_proofs, storage_roots32: *mut u8,
                                           storage_proofs: *mut b200_proofs, opt_stats: *mut b200_stats) -> i32;
+    /// execution witness of a target block on the state after an overlay block (both in the layout of b200_dstate_apply),
+    /// the state unchanged
+    pub fn b200_dstate_overlay_witness(state: *mut b200_dstate, ov_acct_keys32: *const u8, ov_accts: *const b200_account,
+                                       ov_acct_flags: *const u8, ov_m: u64, ov_slot_keys32: *const u8, ov_values32_be: *const u8,
+                                       ov_seg_offsets: *const u64, acct_keys32: *const u8, accts: *const b200_account,
+                                       acct_flags: *const u8, m: u64, slot_keys32: *const u8, values32_be: *const u8,
+                                       seg_offsets: *const u64, mode: i32, always_include_root: i32, overlay_root32: *mut u8,
+                                       out: *mut b200_witness, opt_stats: *mut b200_stats) -> i32;
+    pub fn b200_witness_release(w: *mut b200_witness);
     /// CPUs + preferred memory of the calling thread on the GPU's NUMA node (before allocating staging buffers)
     pub fn b200_numa_bind_thread(device_ordinal: i32) -> i32;
 }

@@ -157,9 +157,10 @@ __device__ __forceinline__ uint32_t ov_root_tree(const DTrieDev &t, uint32_t w) 
 }
 
 // Threads [0, n_blocks): the account root of every block with entries (and the block's parent root for the finish: the
-// current root).  Threads [n_blocks, n_blocks + m): the storage root of every entry that is live, not wiped, has slots and
-// whose account exists with a non-empty storage trie — so the storage tries are revealed at the same levels as the
-// account tries.  found (nullable): found[a] = entry a's account is in the account arena.
+// current root).  Threads [n_blocks, n_blocks + m): the storage root of every entry that is live, not wiped, has slots (or,
+// with reveal_targets, is an account target) and whose account exists with a non-empty storage trie — so the storage tries
+// are revealed at the same levels as the account tries.  found (nullable): found[a] = entry a's account is in the account
+// arena.
 __global__ void ov_seed_kernel(DTrieDev ta, DTrieDev ts, StatelessDev s, const uint8_t *root, uint8_t *parent, OvNode *q,
                                uint32_t *n_q, SlItem *items, uint32_t *n_items, uint8_t *vals, uint8_t *found) {
     const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -174,7 +175,8 @@ __global__ void ov_seed_kernel(DTrieDev ta, DTrieDev ts, StatelessDev s, const u
     const uint64_t a = i - s.n_blocks;
     if (a >= s.m) return;
     const uint32_t fl = sl_flags(s, a);
-    const bool reveal = (fl & 1) && !(fl & 4) && s.seg[a + 1] != s.seg[a];
+    const bool has_slots = s.seg[a + 1] != s.seg[a];
+    const bool reveal = (fl & 1) && !(fl & 4) && (has_slots || s.reveal_targets);
     if (!reveal && !found) return;
     const DtLoc loc = dt_descend(ta, 0, s.akeys + 32 * a);
     if (found) found[a] = loc.found ? 1 : 0;
@@ -182,6 +184,7 @@ __global__ void ov_seed_kernel(DTrieDev ta, DTrieDev ts, StatelessDev s, const u
     const uint32_t w = ts.troot[loc.child & ~DT_LEAF];
     if (w == DT_NONE) return;
     uint32_t tlo = 0, thi = 0;  // the slot targets of the account target with this entry's key
+    bool target = false;
     if (s.n_t) {
         const uint8_t *key = s.akeys + 32 * a;
         uint64_t lo = 0, hi = s.n_t;  // first account target >= key
@@ -193,8 +196,10 @@ __global__ void ov_seed_kernel(DTrieDev ta, DTrieDev ts, StatelessDev s, const u
         if (lo < s.n_t && ov_cmp_nibbles(s.tkeys + 32 * lo, key, 0, 64) == 0) {
             tlo = (uint32_t)s.tseg[lo];
             thi = (uint32_t)s.tseg[lo + 1];
+            target = true;
         }
     }
+    if (!has_slots && !target) return;
     ov_word(ts, s, w, -1, ov_root_tree(ts, w), (uint32_t)a, sl_block_of_entry(s, a), (uint32_t)s.seg[a], (uint32_t)s.seg[a + 1], tlo, thi, q,
             n_q, items, n_items, vals);
 }

@@ -52,14 +52,13 @@ static __device__ void dt_keccak_global(const uint8_t *p, uint32_t len, uint32_t
 // branch at path lkey[..lnib) that the fold did not open.  A target reaches one only where it leaves the extension above
 // that branch: the proof ends with the extension node, whose child is the hash.  A target that shares the whole path
 // would need the branch itself, which the fold does not have: a sticky B200_DEVERR_CORRUPT, never a wrong proof.
+// dt_proof_steps: the walk goes on from child word `cur` below a node at depth pd, adding to n_nodes / n_bytes.  WITNESS, in an arena made
+// from a fold: a hash leaf ends the walk with nothing kept and is returned (the caller continues in the resident arena,
+// tk_witness.cuh); DT_NONE otherwise.
 template <bool WRITE, bool WITNESS = false>
-static __device__ void dt_proof_walk(const DTrieDev &t, uint32_t trie, const uint8_t *key, uint32_t &n_nodes, uint64_t &n_bytes,
-                                     uint8_t *rlp, uint64_t byte_base, uint64_t *rlp_offset, uint8_t *node_depth, uint32_t *node_masks,
-                                     uint64_t node_base, uint32_t min_len = 0, uint32_t stop = 0) {
-    n_nodes = 0;
-    n_bytes = 0;
-    uint32_t cur = t.troot[trie];
-    int pd = -1;
+static __device__ uint32_t dt_proof_steps(const DTrieDev &t, uint32_t cur, int pd, const uint8_t *key, uint32_t &n_nodes, uint64_t &n_bytes,
+                                          uint8_t *rlp, uint64_t byte_base, uint64_t *rlp_offset, uint8_t *node_depth,
+                                          uint32_t *node_masks, uint64_t node_base, uint32_t min_len, uint32_t stop) {
     // depth = number of key nibbles that lead to the node: its path in a ProofNodes / MultiProof map is key[..depth]
     // masks: hash_mask << 16 | tree_mask of a branch node reth would store (BranchNodeMasks), 0 for everything else
     auto begin_node = [&](uint32_t len, int depth, uint32_t masks = 0) {
@@ -73,22 +72,17 @@ static __device__ void dt_proof_walk(const DTrieDev &t, uint32_t trie, const uin
         n_nodes++;
         n_bytes += len;
     };
-    if (cur == DT_NONE) {  // empty trie: the proof is the empty string (EMPTY_STRING_CODE), proof.rs:121-126
-        if (WITNESS && min_len) return;
-        if (WRITE) rlp[byte_base] = 0x80;
-        begin_node(1, 0);
-        return;
-    }
     for (int hops = 0; hops <= DT_MAX_HOPS; hops++) {
         if (cur & DT_LEAF) {
             const uint32_t x = cur & ~DT_LEAF;
+            if (WITNESS && t.lnib && (t.lmeta[x] & META_ISNODE)) return x;
             const uint8_t *val = t.lval + (uint64_t)t.val_stride * x;
             if (!WITNESS && (t.lmeta[x] & META_ISNODE)) {
                 const uint8_t *hk = t.lkey + 32 * (uint64_t)x;
                 const uint32_t L = t.lnib[x];
                 if ((int)L <= pd + 1 || dt_lcp(key, hk, (uint32_t)(pd + 1), L) == L) {
                     atomicExch(t.err, B200_DEVERR_CORRUPT);
-                    return;
+                    return DT_NONE;
                 }
                 uint32_t child[8];
                 for (int w = 0; w < 8; w++)
@@ -101,12 +95,12 @@ static __device__ void dt_proof_walk(const DTrieDev &t, uint32_t trie, const uin
                     encode_extension(lb, hk, (uint32_t)(pd + 1), L, child, 0u);
                 }
                 begin_node(elen, pd + 1);
-                return;
+                return DT_NONE;
             }
             uint32_t k[8];
             load32_nc(t.lkey + 32 * (uint64_t)x, k);
             const uint8_t *sr = t.lsroot ? t.lsroot + 32 * (uint64_t)x : nullptr;
-            if (WITNESS && (uint32_t)(pd + 1) < min_len) return;
+            if (WITNESS && (uint32_t)(pd + 1) < min_len) return DT_NONE;
             CountBuf cb{0};
             uint32_t len = t.account ? encode_leaf<CountBuf, true>(cb, k, pd, val, sr, t.err) : encode_leaf<CountBuf, false>(cb, k, pd, val, nullptr, t.err);
             if (WRITE) {
@@ -115,7 +109,7 @@ static __device__ void dt_proof_walk(const DTrieDev &t, uint32_t trie, const uin
                 else encode_leaf<LinBuf, false>(lb, k, pd, val, nullptr, t.err);
             }
             begin_node(len, pd + 1);
-            return;
+            return DT_NONE;
         }
         const uint32_t v = cur;
         const int d = t.ndepth[v];
@@ -129,7 +123,7 @@ static __device__ void dt_proof_walk(const DTrieDev &t, uint32_t trie, const uin
         const bool matches = dt_lcp(key, nk, (uint32_t)(pd + 1), (uint32_t)d) == (uint32_t)d;
         if (WITNESS && !(ext ? (uint32_t)(pd + 1) >= min_len : (uint32_t)d >= min_len)) {
             // above the wanted depth: walk on without keeping the node
-            if (!matches) return;
+            if (!matches) return DT_NONE;
         } else if (ext) {  // the extension node sits at a prefix of the key (we got here); the branch only if its nibbles match
             uint32_t m = (uint32_t)(d - (pd + 1)), hp_len = 1 + (m >> 1), path_str = hp_len == 1 ? 1 : 1 + hp_len;
             uint32_t clen = blen >= 32 ? 33 : blen;
@@ -154,11 +148,11 @@ static __device__ void dt_proof_walk(const DTrieDev &t, uint32_t trie, const uin
             }
             begin_node(elen, pd + 1);
             if (WITNESS) {
-                if (stop & WT_FIRST_ONLY) return;
+                if (stop & WT_FIRST_ONLY) return DT_NONE;
                 begin_node(blen, d);
-                if (!matches || (stop & (WT_ROOT_ONLY | WT_FIRST_ONLY))) return;
+                if (!matches || (stop & (WT_ROOT_ONLY | WT_FIRST_ONLY))) return DT_NONE;
             } else {
-                if (!matches) return;
+                if (!matches) return DT_NONE;
                 begin_node(blen, d, masks);
             }
         } else {
@@ -167,13 +161,36 @@ static __device__ void dt_proof_walk(const DTrieDev &t, uint32_t trie, const uin
                 dt_put_branch<false>(br, t, v, payload);
             }
             begin_node(blen, d, masks);
-            if (WITNESS && (stop & (WT_ROOT_ONLY | WT_FIRST_ONLY))) return;
+            if (WITNESS && (stop & (WT_ROOT_ONLY | WT_FIRST_ONLY))) return DT_NONE;
         }
         pd = d;
         cur = t.nchild[16 * (uint64_t)v + dt_nib(key, (uint32_t)d)];
-        if (cur == DT_NONE) return;  // exclusion: the branch has no child for the key's next nibble
+        if (cur == DT_NONE) return DT_NONE;  // exclusion: the branch has no child for the key's next nibble
     }
     atomicExch(t.err, B200_DEVERR_CORRUPT);
+    return DT_NONE;
+}
+template <bool WRITE, bool WITNESS = false>
+static __device__ uint32_t dt_proof_walk(const DTrieDev &t, uint32_t trie, const uint8_t *key, uint32_t &n_nodes, uint64_t &n_bytes,
+                                         uint8_t *rlp, uint64_t byte_base, uint64_t *rlp_offset, uint8_t *node_depth, uint32_t *node_masks,
+                                         uint64_t node_base, uint32_t min_len = 0, uint32_t stop = 0) {
+    n_nodes = 0;
+    n_bytes = 0;
+    const uint32_t cur = t.troot[trie];
+    if (cur == DT_NONE) {  // empty trie: the proof is the empty string (EMPTY_STRING_CODE), proof.rs:121-126
+        if (WITNESS && min_len) return DT_NONE;
+        if (WRITE) rlp[byte_base] = 0x80;
+        n_nodes = 1;
+        n_bytes = 1;
+        if (WRITE) rlp_offset[node_base] = byte_base;
+        if (WRITE && !WITNESS) {
+            node_depth[node_base] = 0;
+            node_masks[node_base] = 0;
+        }
+        return DT_NONE;
+    }
+    return dt_proof_steps<WRITE, WITNESS>(t, cur, -1, key, n_nodes, n_bytes, rlp, byte_base, rlp_offset, node_depth, node_masks, node_base,
+                                          min_len, stop);
 }
 
 // trie_of_target: nullptr = trie 0 of t; DT_NONE entries (storage of an absent account) prove against the empty trie;
@@ -224,7 +241,7 @@ __global__ void dt_find_leaf_kernel(DTrieDev t, const uint8_t *__restrict__ key,
 
 // ---- multiproof batch (MultiProofTargets: accounts with their slot targets)
 // leaf_out[i] = the account leaf (= storage trie id) of account key i, DT_NONE when the account does not exist; its storage
-// root goes to sroot_out (EMPTY_ROOT_HASH for a missing account)
+// root goes to sroot_out (nullable; EMPTY_ROOT_HASH for a missing account)
 __global__ void dt_find_leaves_kernel(DTrieDev t, const uint8_t *__restrict__ keys, uint64_t n, uint32_t *__restrict__ leaf_out,
                                       uint8_t *__restrict__ sroot_out) {
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -233,6 +250,7 @@ __global__ void dt_find_leaves_kernel(DTrieDev t, const uint8_t *__restrict__ ke
     DtLoc loc = dt_descend(t, t.ltrie ? (uint32_t)(key[0] >> 4) : 0u, key);
     uint32_t leaf = loc.found ? (loc.child & ~DT_LEAF) : DT_NONE;
     leaf_out[i] = leaf;
+    if (!sroot_out) return;
     if (leaf != DT_NONE && t.lsroot) dt_copy32(sroot_out + 32 * i, t.lsroot + 32 * (uint64_t)leaf);
     else dt_put_empty_root(sroot_out + 32 * i);
 }

@@ -15,6 +15,12 @@
 //     emits the proof target (key = path ‖ c ‖ 0…0, min_len = |path ‖ c|): what the sparse trie's blinded-node callback
 //     asks for (crates/trie/sparse/src/parallel.rs:1004-1013).
 // Per-node scratch: two words per node slot of the arena, cleared for every call.
+//
+// b200_dstate_overlay_witness runs the same kernels on the folds of an overlay (da_from_fold): every target path is opened
+// there, and a hash leaf (lmeta META_ISNODE: an unchanged resident subtree) counts as a surviving, hashed, unseen child.
+// The walks that go below a hash leaf (the branch under a diverging extension, a collapse sibling, the leaves of a wiped
+// storage) carry on, read-only, in the resident arena of the same trie (wt_fall).  Storage trie ids are then the overlay's
+// entries (entry_trie), and res_trie[trie] names the resident storage trie behind one.
 
 static __device__ __forceinline__ uint32_t wt_child_mask(const DTrieDev &t, uint32_t v) {
     uint32_t m = 0;
@@ -79,6 +85,44 @@ static __device__ __forceinline__ bool wt_account_empty(const uint8_t *a) {
     return true;
 }
 
+// The resident branch behind hash leaf x of fold arena f: the node of resident trie rt at depth lnib[x] on the path lkey[x],
+// whose own hash must be the one the leaf holds (nref is the reference its resident parent holds: below an implicit
+// extension that is the extension's, so the branch is re-hashed).  Anything else latches B200_DEVERR_CORRUPT: DT_NONE.
+static __device__ uint32_t wt_fall(const DTrieDev &f, uint32_t x, const DTrieDev &r, uint32_t rt) {
+    const uint8_t *hk = f.lkey + 32 * (uint64_t)x, *want = f.lval + (uint64_t)f.val_stride * x;
+    const uint32_t L = f.lnib[x];
+    uint32_t cur = rt == DT_NONE ? DT_NONE : r.troot[rt];
+    int pd = -1;
+    for (int hops = 0; hops <= DT_MAX_HOPS && cur != DT_NONE && !(cur & DT_LEAF); hops++) {
+        const uint32_t d = r.ndepth[cur];
+        if (d > L || dt_lcp(hk, r.nkey + 32 * (uint64_t)cur, (uint32_t)(pd + 1), d) < d) break;
+        if (d < L) {
+            pd = (int)d;
+            cur = r.nchild[16 * (uint64_t)cur + dt_nib(hk, d)];
+            continue;
+        }
+        bool same = true;
+        if (pd + 1 == (int)L) {
+            for (int k = 0; k < 32; k++) same &= r.nref[32 * (uint64_t)cur + k] == want[k];
+        } else {
+            uint32_t sm, tm, hm, dig[8];
+            const uint32_t payload = dt_branch_payload<false>(r, cur, sm, tm, hm), blen = list_header_len(payload) + payload;
+            uint8_t br[544];
+            LinBuf lb{br, 0};
+            dt_put_branch<false>(lb, r, cur, payload);
+            dt_keccak_global(br, blen, dig);
+            for (int k = 0; k < 32; k++) same &= (uint8_t)(dig[k >> 2] >> (8 * (k & 3))) == want[k];
+        }
+        if (same) return cur;
+        break;
+    }
+    atomicExch(f.err, B200_DEVERR_CORRUPT);
+    return DT_NONE;
+}
+static __device__ __forceinline__ bool wt_hash_leaf(const DTrieDev &t, uint32_t w) {
+    return (w & DT_LEAF) && t.lnib && (t.lmeta[w & ~DT_LEAF] & META_ISNODE);
+}
+
 static __device__ __forceinline__ uint32_t wt_account_of(const uint64_t *__restrict__ seg_offsets, uint64_t m, uint64_t j) {
     uint64_t lo = 0, hi = m;  // last account with offset <= j
     while (hi - lo > 1) {
@@ -92,9 +136,11 @@ static __device__ __forceinline__ bool wt_wiped(const uint8_t *flags, uint64_t i
     return flags != nullptr && (!(flags[i] & 1) || (flags[i] & 4));
 }
 
-// Accounts, first pass: the leaf (= storage trie id) of every account entry, the key order, the wiped storage tries.
+// Accounts, first pass: the account leaf and the storage trie (entry_trie, nullable: the leaf) of every account entry, the
+// key order, the wiped storage tries.
 __global__ void wt_accounts_kernel(DTrieDev ta, DTrieDev ts, const uint8_t *__restrict__ keys, const uint8_t *__restrict__ flags,
-                                   uint64_t m, uint32_t *__restrict__ leaf_of, uint8_t *__restrict__ trie_flags) {
+                                   uint64_t m, const uint32_t *__restrict__ entry_trie, uint32_t *__restrict__ leaf_of,
+                                   uint32_t *__restrict__ trie_of, uint8_t *__restrict__ trie_flags) {
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= m) return;
     const uint8_t *key = keys + 32 * i;
@@ -104,14 +150,16 @@ __global__ void wt_accounts_kernel(DTrieDev ta, DTrieDev ts, const uint8_t *__re
     }
     DtLoc loc = dt_descend(ta, 0, key);
     const uint32_t leaf = loc.found ? (loc.child & ~DT_LEAF) : DT_NONE;
+    const uint32_t trie = leaf == DT_NONE ? DT_NONE : entry_trie ? entry_trie[i] : leaf;
     leaf_of[i] = leaf;
-    if (leaf != DT_NONE && wt_wiped(flags, i) && ts.troot[leaf] != DT_NONE) trie_flags[leaf] = WF_WIPED;
+    trie_of[i] = trie;
+    if (trie != DT_NONE && wt_wiped(flags, i) && ts.troot[trie] != DT_NONE) trie_flags[trie] = WF_WIPED;
 }
 
 // Slot entries: the storage target j (trie, key), the key order, and the walk of every entry of a storage trie that is not
 // wiped (a wiped trie loses every leaf: no branch of it keeps a pre-state child, so it reveals nothing).
 __global__ void wt_slots_kernel(DTrieDev ts, WitnessMarks w, const uint64_t *__restrict__ seg_offsets, uint64_t m,
-                                const uint32_t *__restrict__ leaf_of, const uint8_t *__restrict__ flags,
+                                const uint32_t *__restrict__ trie_of, const uint8_t *__restrict__ flags,
                                 const uint8_t *__restrict__ keys, const uint8_t *__restrict__ vals, uint64_t n, int canonical,
                                 uint32_t *__restrict__ trie_of_target, uint8_t *__restrict__ nonzero) {
     uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -125,7 +173,7 @@ __global__ void wt_slots_kernel(DTrieDev ts, WitnessMarks w, const uint64_t *__r
     const uint64_t *v = reinterpret_cast<const uint64_t *>(vals + 32 * j);
     const bool upsert = (v[0] | v[1] | v[2] | v[3]) != 0;
     if (upsert) nonzero[i] = 1;
-    const uint32_t trie = leaf_of[i];
+    const uint32_t trie = trie_of[i];
     trie_of_target[j] = trie;
     if (trie == DT_NONE || wt_wiped(flags, i)) return;
     const bool found = wt_walk(ts, w, trie, key, !upsert, false);
@@ -137,17 +185,17 @@ __global__ void wt_slots_kernel(DTrieDev ts, WitnessMarks w, const uint64_t *__r
 __global__ void wt_account_walk_kernel(DTrieDev ta, DTrieDev ts, WitnessMarks w, const uint8_t *__restrict__ keys,
                                        const uint8_t *__restrict__ accts, const uint8_t *__restrict__ flags,
                                        const uint64_t *__restrict__ seg_offsets, uint64_t m, const uint32_t *__restrict__ leaf_of,
-                                       const uint8_t *__restrict__ trie_flags, const uint8_t *__restrict__ nonzero, int canonical,
+                                       const uint32_t *__restrict__ trie_of, const uint8_t *__restrict__ trie_flags, const uint8_t *__restrict__ nonzero, int canonical,
                                        uint32_t *__restrict__ root_trie, uint16_t *__restrict__ root_meta) {
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= m) return;
-    const uint32_t leaf = leaf_of[i];
+    const uint32_t leaf = leaf_of[i], trie = trie_of[i];
     const uint8_t f = flags ? flags[i] : 1;
     const bool wiped = wt_wiped(flags, i);
-    const bool pre_empty = leaf == DT_NONE || ts.troot[leaf] == DT_NONE;
+    const bool pre_empty = trie == DT_NONE || ts.troot[trie] == DT_NONE;
     const bool has_targets = seg_offsets[i + 1] > seg_offsets[i] || (wiped && !pre_empty);
     bool post_empty;
-    if (has_targets) post_empty = (pre_empty || wiped || (trie_flags[leaf] & WF_EMPTIED)) && !nonzero[i];
+    if (has_targets) post_empty = (pre_empty || wiped || (trie_flags[trie] & WF_EMPTIED)) && !nonzero[i];
     else post_empty = pre_empty;
     // as b200_dstate_apply does: a destroyed account goes whatever its slot entries say, and an "unchanged" entry of an
     // absent account is ignored with its slots (its key is still a target: its proof shows the absence)
@@ -157,7 +205,7 @@ __global__ void wt_account_walk_kernel(DTrieDev ta, DTrieDev ts, WitnessMarks w,
     else if (ignored) removal = false;
     else if (f & 2) removal = wt_account_empty(ta.lval + 72 * (uint64_t)leaf) && post_empty;  // unchanged: the resident one
     else removal = wt_account_empty(accts + 72 * i) && post_empty;
-    root_trie[i] = leaf;
+    root_trie[i] = trie;
     root_meta[i] = (!canonical && !has_targets) ? WM_ROOT_ONLY : WM_SKIP;
     const bool found = wt_walk(ta, w, 0, keys + 32 * i, removal, false);
     if (canonical && !removal && !ignored && !found) wt_walk(ta, w, 0, keys + 32 * i, false, true);
@@ -174,7 +222,9 @@ __global__ void wt_reveal_kernel(DTrieDev t, WitnessMarks w, uint32_t max_list, 
     if (__popc(surv) != 1 || (seen & surv)) return;
     const uint32_t c = __ffs(surv) - 1, d = t.ndepth[v], child = t.nchild[16 * (uint64_t)v + c];
     uint32_t len;
-    if (child & DT_LEAF) {
+    if (wt_hash_leaf(t, child)) {
+        len = 32;  // an unopened branch of at least 32 bytes, or the extension above one
+    } else if (child & DT_LEAF) {
         const uint32_t x = child & ~DT_LEAF;
         uint32_t k[8];
         load32_nc(t.lkey + 32 * (uint64_t)x, k);
@@ -208,52 +258,68 @@ __global__ void wt_reveal_kernel(DTrieDev t, WitnessMarks w, uint32_t max_list, 
 
 // Wipe expansion: a read-only breadth-first walk of the wiped storage tries (the traversal of the apply's release path,
 // dt_wipe_*_kernel, on a queue of its own), so its cost follows the size of those tries, not of the arena.  Every live leaf
-// of a wiped trie becomes a storage target.
+// of a wiped trie becomes a storage target.  A queue entry is a pair (node, trie): the node is one of ts, or with DT_ALT one
+// of res, the resident arena below a hash leaf of a fold; the trie is ts's, the one its leaves prove in.
+static __device__ __forceinline__ void wt_wipe_push(uint32_t *queue, uint32_t *n_queue, uint32_t node, uint32_t trie) {
+    const uint32_t k = atomicAdd(n_queue, 1u);
+    queue[2 * (uint64_t)k] = node;
+    queue[2 * (uint64_t)k + 1] = trie;
+}
+// child word w of a wiped trie (alt: a word of res): a node is queued, a leaf counted, a hash leaf queues the branch behind it
+static __device__ void wt_wipe_child(const DTrieDev &ts, const DTrieDev &res, const uint32_t *res_trie, uint32_t w, uint32_t trie,
+                                     uint32_t alt, uint32_t *queue, uint32_t *n_queue, uint32_t *n_leaves) {
+    if (w == DT_NONE) return;
+    if (!alt && wt_hash_leaf(ts, w)) {
+        const uint32_t r = wt_fall(ts, w & ~DT_LEAF, res, res_trie ? res_trie[trie] : 0u);
+        if (r != DT_NONE) wt_wipe_push(queue, n_queue, r | DT_ALT, trie);
+    } else if (w & DT_LEAF) {
+        atomicAdd(n_leaves, 1u);
+    } else {
+        wt_wipe_push(queue, n_queue, w | alt, trie);
+    }
+}
 // roots: a leaf root is counted (WRITE: written as a target); a node root is queued (count pass only)
 template <bool WRITE>
-__global__ void wt_wipe_roots_kernel(DTrieDev ts, const uint32_t *__restrict__ leaf_of, const uint8_t *__restrict__ trie_flags, uint64_t m,
-                                     uint32_t *__restrict__ queue, uint32_t *__restrict__ n_queue, uint32_t *__restrict__ n_out,
-                                     uint32_t *__restrict__ out_trie, uint8_t *__restrict__ out_keys) {
+__global__ void wt_wipe_roots_kernel(DTrieDev ts, DTrieDev res, const uint32_t *__restrict__ res_trie, const uint32_t *__restrict__ trie_of,
+                                     const uint8_t *__restrict__ trie_flags, uint64_t m, uint32_t *__restrict__ queue,
+                                     uint32_t *__restrict__ n_queue, uint32_t *__restrict__ n_out, uint32_t *__restrict__ out_trie,
+                                     uint8_t *__restrict__ out_keys) {
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= m) return;
-    const uint32_t trie = leaf_of[i];
+    const uint32_t trie = trie_of[i];
     if (trie == DT_NONE || !(trie_flags[trie] & WF_WIPED)) return;
     const uint32_t w = ts.troot[trie];
-    if (w & DT_LEAF) {
+    if (!WRITE) {
+        wt_wipe_child(ts, res, res_trie, w, trie, 0u, queue, n_queue, n_out);
+    } else if ((w & DT_LEAF) && !wt_hash_leaf(ts, w)) {
         const uint32_t o = atomicAdd(n_out, 1u);
-        if (WRITE) {
-            out_trie[o] = trie;
-            dt_copy32(out_keys + 32 * (uint64_t)o, ts.lkey + 32 * (uint64_t)(w & ~DT_LEAF));
-        }
-    } else if (!WRITE) {
-        queue[atomicAdd(n_queue, 1u)] = w;
+        out_trie[o] = trie;
+        dt_copy32(out_keys + 32 * (uint64_t)o, ts.lkey + 32 * (uint64_t)(w & ~DT_LEAF));
     }
 }
 // one level: queue[lo, hi) was pushed by the level before; child nodes are queued, child leaves counted
-__global__ void wt_wipe_round_kernel(DTrieDev ts, uint32_t *__restrict__ queue, uint32_t lo, uint32_t hi, uint32_t *__restrict__ n_queue,
-                                     uint32_t *__restrict__ n_leaves) {
+__global__ void wt_wipe_round_kernel(DTrieDev ts, DTrieDev res, const uint32_t *__restrict__ res_trie, uint32_t *__restrict__ queue,
+                                     uint32_t lo, uint32_t hi, uint32_t *__restrict__ n_queue, uint32_t *__restrict__ n_leaves) {
     uint32_t i = lo + blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= hi) return;
-    const uint32_t *ch = ts.nchild + 16 * (uint64_t)queue[i];
-    for (int s = 0; s < 16; s++) {
-        const uint32_t w = ch[s];
-        if (w == DT_NONE) continue;
-        if (w & DT_LEAF) atomicAdd(n_leaves, 1u);
-        else queue[atomicAdd(n_queue, 1u)] = w;
-    }
+    const uint32_t v = queue[2 * (uint64_t)i], trie = queue[2 * (uint64_t)i + 1], alt = v & DT_ALT;
+    const uint32_t *ch = (alt ? res.nchild : ts.nchild) + 16 * (uint64_t)(v & ~DT_ALT);
+    for (int s = 0; s < 16; s++) wt_wipe_child(ts, res, res_trie, ch[s], trie, alt, queue, n_queue, n_leaves);
 }
 // every node the walk queued writes its leaf children as targets
-__global__ void wt_wipe_leaves_kernel(DTrieDev ts, const uint32_t *__restrict__ queue, uint32_t n, uint32_t *__restrict__ n_out,
+__global__ void wt_wipe_leaves_kernel(DTrieDev ts, DTrieDev res, const uint32_t *__restrict__ queue, uint32_t n, uint32_t *__restrict__ n_out,
                                       uint32_t *__restrict__ out_trie, uint8_t *__restrict__ out_keys) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const uint32_t v = queue[i], *ch = ts.nchild + 16 * (uint64_t)v;
+    const uint32_t v = queue[2 * (uint64_t)i], trie = queue[2 * (uint64_t)i + 1], alt = v & DT_ALT;
+    const uint32_t *ch = (alt ? res.nchild : ts.nchild) + 16 * (uint64_t)(v & ~DT_ALT);
+    const uint8_t *lkey = alt ? res.lkey : ts.lkey;
     for (int s = 0; s < 16; s++) {
         const uint32_t w = ch[s];
-        if (w == DT_NONE || !(w & DT_LEAF)) continue;
+        if (w == DT_NONE || !(w & DT_LEAF) || (!alt && wt_hash_leaf(ts, w))) continue;
         const uint32_t o = atomicAdd(n_out, 1u);
-        out_trie[o] = ts.ntrie[v];
-        dt_copy32(out_keys + 32 * (uint64_t)o, ts.lkey + 32 * (uint64_t)(w & ~DT_LEAF));
+        out_trie[o] = trie;
+        dt_copy32(out_keys + 32 * (uint64_t)o, lkey + 32 * (uint64_t)(w & ~DT_LEAF));
     }
 }
 
@@ -279,9 +345,11 @@ __global__ void wt_clear_kernel(DTrieDev t, WitnessMarks w, const uint32_t *__re
     }
 }
 
-// Proof walks of the targets [0, n_fixed + *n_extra) (meta: min_len | stop bits; trie DT_NONE = the empty trie).
+// Proof walks of the targets [0, n_fixed + *n_extra) (meta: min_len | stop bits; trie DT_NONE = the empty trie).  A walk
+// that reaches a hash leaf of a fold goes on in res, in trie res_trie[trie] (nullptr: trie 0).
 template <bool WRITE>
-static __device__ __forceinline__ void wt_target(const DTrieDev &t, const uint32_t *__restrict__ trie_of, const uint8_t *__restrict__ keys,
+static __device__ __forceinline__ void wt_target(const DTrieDev &t, const DTrieDev &res, const uint32_t *__restrict__ res_trie,
+                                                 const uint32_t *__restrict__ trie_of, const uint8_t *__restrict__ keys,
                                                  const uint16_t *__restrict__ meta, uint64_t i, uint32_t &nn, uint64_t &nb,
                                                  uint8_t *rlp, uint64_t byte_base, uint64_t *rlp_offset, uint64_t node_base) {
     const uint32_t trie = trie_of ? trie_of[i] : 0;
@@ -300,21 +368,26 @@ static __device__ __forceinline__ void wt_target(const DTrieDev &t, const uint32
         }
         return;
     }
-    dt_proof_walk<WRITE, true>(t, trie, keys + 32 * i, nn, nb, rlp, byte_base, rlp_offset, nullptr, nullptr, node_base, mt & 0xFF,
-                               mt >> 8);
+    const uint32_t x = dt_proof_walk<WRITE, true>(t, trie, keys + 32 * i, nn, nb, rlp, byte_base, rlp_offset, nullptr, nullptr, node_base,
+                                                  mt & 0xFF, mt >> 8);
+    if (x == DT_NONE) return;
+    const uint32_t r = wt_fall(t, x, res, res_trie ? res_trie[trie] : 0u), p = t.lparent[x];
+    if (r != DT_NONE)
+        dt_proof_steps<WRITE, true>(res, r, p == DT_NONE ? -1 : (int)t.ndepth[p], keys + 32 * i, nn, nb, rlp, byte_base, rlp_offset, nullptr,
+                                    nullptr, node_base, mt & 0xFF, mt >> 8);
 }
-__global__ void wt_proof_size_kernel(DTrieDev t, const uint32_t *__restrict__ trie_of, const uint8_t *__restrict__ keys,
+__global__ void wt_proof_size_kernel(DTrieDev t, DTrieDev res, const uint32_t *__restrict__ res_trie, const uint32_t *__restrict__ trie_of, const uint8_t *__restrict__ keys,
                                      const uint16_t *__restrict__ meta, uint64_t n_fixed, const uint32_t *__restrict__ n_extra, uint64_t n_max,
                                      uint32_t *__restrict__ node_count, uint64_t *__restrict__ byte_count) {
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n_max) return;
     uint32_t nn = 0;
     uint64_t nb = 0;
-    if (i < n_fixed + (n_extra ? *n_extra : 0u)) wt_target<false>(t, trie_of, keys, meta, i, nn, nb, nullptr, 0, nullptr, 0);
+    if (i < n_fixed + (n_extra ? *n_extra : 0u)) wt_target<false>(t, res, res_trie, trie_of, keys, meta, i, nn, nb, nullptr, 0, nullptr, 0);
     node_count[i] = nn;
     byte_count[i] = nb;
 }
-__global__ void wt_proof_write_kernel(DTrieDev t, const uint32_t *__restrict__ trie_of, const uint8_t *__restrict__ keys,
+__global__ void wt_proof_write_kernel(DTrieDev t, DTrieDev res, const uint32_t *__restrict__ res_trie, const uint32_t *__restrict__ trie_of, const uint8_t *__restrict__ keys,
                                       const uint16_t *__restrict__ meta, uint64_t n_fixed, const uint32_t *__restrict__ n_extra,
                                       uint64_t n_max, const uint64_t *__restrict__ node_base, const uint64_t *__restrict__ byte_base,
                                       uint64_t node_shift, uint64_t byte_shift, uint8_t *__restrict__ rlp, uint64_t *__restrict__ rlp_offset) {
@@ -322,7 +395,7 @@ __global__ void wt_proof_write_kernel(DTrieDev t, const uint32_t *__restrict__ t
     if (i >= n_max || i >= n_fixed + (n_extra ? *n_extra : 0u)) return;
     uint32_t nn;
     uint64_t nb;
-    wt_target<true>(t, trie_of, keys, meta, i, nn, nb, rlp, byte_shift + byte_base[i], rlp_offset, node_shift + node_base[i]);
+    wt_target<true>(t, res, res_trie, trie_of, keys, meta, i, nn, nb, rlp, byte_shift + byte_base[i], rlp_offset, node_shift + node_base[i]);
 }
 
 // After the sort by hash: keep[i] = 1 for the first of every run of equal hashes (Canonical: not the empty node 0x80),
@@ -359,22 +432,22 @@ __global__ void wt_gather_kernel(const uint8_t *__restrict__ sorted32, const uin
 
 // ------------------------------------------------------------------------------------------------ launchers
 cudaError_t launch_wt_accounts(const DTrieDev &ta, const DTrieDev &ts, const uint8_t *keys, const uint8_t *flags, uint64_t m,
-                               uint32_t *leaf_of, uint8_t *trie_flags, cudaStream_t st) {
-    if (m) wt_accounts_kernel<<<blocks_for(m, 128), 128, 0, st>>>(ta, ts, keys, flags, m, leaf_of, trie_flags);
+                               const uint32_t *entry_trie, uint32_t *leaf_of, uint32_t *trie_of, uint8_t *trie_flags, cudaStream_t st) {
+    if (m) wt_accounts_kernel<<<blocks_for(m, 128), 128, 0, st>>>(ta, ts, keys, flags, m, entry_trie, leaf_of, trie_of, trie_flags);
     return cudaGetLastError();
 }
-cudaError_t launch_wt_slots(const DTrieDev &ts, const WitnessMarks &w, const uint64_t *seg_offsets, uint64_t m, const uint32_t *leaf_of,
+cudaError_t launch_wt_slots(const DTrieDev &ts, const WitnessMarks &w, const uint64_t *seg_offsets, uint64_t m, const uint32_t *trie_of,
                             const uint8_t *flags, const uint8_t *keys, const uint8_t *vals, uint64_t n, int canonical,
                             uint32_t *trie_of_target, uint8_t *nonzero, cudaStream_t st) {
-    if (n) wt_slots_kernel<<<blocks_for(n, 128), 128, 0, st>>>(ts, w, seg_offsets, m, leaf_of, flags, keys, vals, n, canonical, trie_of_target, nonzero);
+    if (n) wt_slots_kernel<<<blocks_for(n, 128), 128, 0, st>>>(ts, w, seg_offsets, m, trie_of, flags, keys, vals, n, canonical, trie_of_target, nonzero);
     return cudaGetLastError();
 }
 cudaError_t launch_wt_account_walk(const DTrieDev &ta, const DTrieDev &ts, const WitnessMarks &w, const uint8_t *keys, const uint8_t *accts,
                                    const uint8_t *flags, const uint64_t *seg_offsets, uint64_t m, const uint32_t *leaf_of,
-                                   const uint8_t *trie_flags, const uint8_t *nonzero, int canonical, uint32_t *root_trie,
+                                   const uint32_t *trie_of, const uint8_t *trie_flags, const uint8_t *nonzero, int canonical, uint32_t *root_trie,
                                    uint16_t *root_meta, cudaStream_t st) {
     if (m)
-        wt_account_walk_kernel<<<blocks_for(m, 128), 128, 0, st>>>(ta, ts, w, keys, accts, flags, seg_offsets, m, leaf_of, trie_flags, nonzero,
+        wt_account_walk_kernel<<<blocks_for(m, 128), 128, 0, st>>>(ta, ts, w, keys, accts, flags, seg_offsets, m, leaf_of, trie_of, trie_flags, nonzero,
                                                                    canonical, root_trie, root_meta);
     return cudaGetLastError();
 }
@@ -383,21 +456,26 @@ cudaError_t launch_wt_reveal(const DTrieDev &t, const WitnessMarks &w, uint32_t 
     if (max_list) wt_reveal_kernel<<<blocks_for(max_list, 128), 128, 0, st>>>(t, w, max_list, canonical, out_trie, out_keys, out_meta, n_out);
     return cudaGetLastError();
 }
-cudaError_t launch_wt_wipe_roots(const DTrieDev &ts, const uint32_t *leaf_of, const uint8_t *trie_flags, uint64_t m, bool write,
-                                 uint32_t *queue, uint32_t *n_queue, uint32_t *n_out, uint32_t *out_trie, uint8_t *out_keys, cudaStream_t st) {
+cudaError_t launch_wt_wipe_roots(const DTrieDev &ts, const DTrieDev &res, const uint32_t *res_trie, const uint32_t *trie_of,
+                                 const uint8_t *trie_flags, uint64_t m, bool write, uint32_t *queue, uint32_t *n_queue, uint32_t *n_out,
+                                 uint32_t *out_trie, uint8_t *out_keys, cudaStream_t st) {
     if (!m) return cudaSuccess;
-    if (write) wt_wipe_roots_kernel<true><<<blocks_for(m, 128), 128, 0, st>>>(ts, leaf_of, trie_flags, m, queue, n_queue, n_out, out_trie, out_keys);
-    else wt_wipe_roots_kernel<false><<<blocks_for(m, 128), 128, 0, st>>>(ts, leaf_of, trie_flags, m, queue, n_queue, n_out, out_trie, out_keys);
+    if (write)
+        wt_wipe_roots_kernel<true><<<blocks_for(m, 128), 128, 0, st>>>(ts, res, res_trie, trie_of, trie_flags, m, queue, n_queue, n_out, out_trie,
+                                                                        out_keys);
+    else
+        wt_wipe_roots_kernel<false><<<blocks_for(m, 128), 128, 0, st>>>(ts, res, res_trie, trie_of, trie_flags, m, queue, n_queue, n_out, out_trie,
+                                                                         out_keys);
     return cudaGetLastError();
 }
-cudaError_t launch_wt_wipe_round(const DTrieDev &ts, uint32_t *queue, uint32_t lo, uint32_t hi, uint32_t *n_queue, uint32_t *n_leaves,
-                                 cudaStream_t st) {
-    if (hi > lo) wt_wipe_round_kernel<<<blocks_for(hi - lo, 128), 128, 0, st>>>(ts, queue, lo, hi, n_queue, n_leaves);
+cudaError_t launch_wt_wipe_round(const DTrieDev &ts, const DTrieDev &res, const uint32_t *res_trie, uint32_t *queue, uint32_t lo, uint32_t hi,
+                                 uint32_t *n_queue, uint32_t *n_leaves, cudaStream_t st) {
+    if (hi > lo) wt_wipe_round_kernel<<<blocks_for(hi - lo, 128), 128, 0, st>>>(ts, res, res_trie, queue, lo, hi, n_queue, n_leaves);
     return cudaGetLastError();
 }
-cudaError_t launch_wt_wipe_leaves(const DTrieDev &ts, const uint32_t *queue, uint32_t n, uint32_t *n_out, uint32_t *out_trie,
-                                  uint8_t *out_keys, cudaStream_t st) {
-    if (n) wt_wipe_leaves_kernel<<<blocks_for(n, 128), 128, 0, st>>>(ts, queue, n, n_out, out_trie, out_keys);
+cudaError_t launch_wt_wipe_leaves(const DTrieDev &ts, const DTrieDev &res, const uint32_t *queue, uint32_t n, uint32_t *n_out,
+                                  uint32_t *out_trie, uint8_t *out_keys, cudaStream_t st) {
+    if (n) wt_wipe_leaves_kernel<<<blocks_for(n, 128), 128, 0, st>>>(ts, res, queue, n, n_out, out_trie, out_keys);
     return cudaGetLastError();
 }
 cudaError_t launch_wt_clear(const DTrieDev &t, const WitnessMarks &w, const uint32_t *trie_of, const uint8_t *keys, uint64_t n,
@@ -405,16 +483,17 @@ cudaError_t launch_wt_clear(const DTrieDev &t, const WitnessMarks &w, const uint
     if (n) wt_clear_kernel<<<blocks_for(n, 128), 128, 0, st>>>(t, w, trie_of, keys, n, leaf_of, trie_flags);
     return cudaGetLastError();
 }
-cudaError_t launch_wt_proof_sizes(const DTrieDev &t, const uint32_t *trie_of, const uint8_t *keys, const uint16_t *meta, uint64_t n_fixed,
+cudaError_t launch_wt_proof_sizes(const DTrieDev &t, const DTrieDev &res, const uint32_t *res_trie, const uint32_t *trie_of, const uint8_t *keys, const uint16_t *meta, uint64_t n_fixed,
                                   const uint32_t *n_extra, uint64_t n_max, uint32_t *node_count, uint64_t *byte_count, cudaStream_t st) {
-    if (n_max) wt_proof_size_kernel<<<blocks_for(n_max, 64), 64, 0, st>>>(t, trie_of, keys, meta, n_fixed, n_extra, n_max, node_count, byte_count);
+    if (n_max) wt_proof_size_kernel<<<blocks_for(n_max, 64), 64, 0, st>>>(t, res, res_trie, trie_of, keys, meta, n_fixed, n_extra, n_max, node_count,
+                                                                   byte_count);
     return cudaGetLastError();
 }
-cudaError_t launch_wt_proof_write(const DTrieDev &t, const uint32_t *trie_of, const uint8_t *keys, const uint16_t *meta, uint64_t n_fixed,
+cudaError_t launch_wt_proof_write(const DTrieDev &t, const DTrieDev &res, const uint32_t *res_trie, const uint32_t *trie_of, const uint8_t *keys, const uint16_t *meta, uint64_t n_fixed,
                                   const uint32_t *n_extra, uint64_t n_max, const uint64_t *node_base, const uint64_t *byte_base,
                                   uint64_t node_shift, uint64_t byte_shift, uint8_t *rlp, uint64_t *rlp_offset, cudaStream_t st) {
     if (n_max)
-        wt_proof_write_kernel<<<blocks_for(n_max, 64), 64, 0, st>>>(t, trie_of, keys, meta, n_fixed, n_extra, n_max, node_base, byte_base,
+        wt_proof_write_kernel<<<blocks_for(n_max, 64), 64, 0, st>>>(t, res, res_trie, trie_of, keys, meta, n_fixed, n_extra, n_max, node_base, byte_base,
                                                                     node_shift, byte_shift, rlp, rlp_offset);
     return cudaGetLastError();
 }

@@ -288,30 +288,37 @@ struct WitnessMarks {       // per-call scratch of one arena
     uint32_t *n_list;
     uint8_t *trie_flags;    // storage forest only, [account leaf capacity]: WF_*
 };
+// b200_dstate_overlay_witness runs these on an overlay's folds: entry_trie (nullable: the account leaf) is the storage trie of
+// every entry; res / res_trie: the resident arena, and its trie behind each trie of the fold, below the fold's hash leaves
+// (res_trie nullptr: trie 0).  On the resident arenas res is the arena itself and holds no hash leaf.
 cudaError_t launch_wt_accounts(const DTrieDev &ta, const DTrieDev &ts, const uint8_t *keys, const uint8_t *flags, uint64_t m,
-                               uint32_t *leaf_of, uint8_t *trie_flags, cudaStream_t st);
-cudaError_t launch_wt_slots(const DTrieDev &ts, const WitnessMarks &w, const uint64_t *seg_offsets, uint64_t m, const uint32_t *leaf_of,
+                               const uint32_t *entry_trie, uint32_t *leaf_of, uint32_t *trie_of, uint8_t *trie_flags, cudaStream_t st);
+cudaError_t launch_wt_slots(const DTrieDev &ts, const WitnessMarks &w, const uint64_t *seg_offsets, uint64_t m, const uint32_t *trie_of,
                             const uint8_t *flags, const uint8_t *keys, const uint8_t *vals, uint64_t n, int canonical,
                             uint32_t *trie_of_target, uint8_t *nonzero, cudaStream_t st);
 cudaError_t launch_wt_account_walk(const DTrieDev &ta, const DTrieDev &ts, const WitnessMarks &w, const uint8_t *keys, const uint8_t *accts,
                                    const uint8_t *flags, const uint64_t *seg_offsets, uint64_t m, const uint32_t *leaf_of,
-                                   const uint8_t *trie_flags, const uint8_t *nonzero, int canonical, uint32_t *root_trie,
-                                   uint16_t *root_meta, cudaStream_t st);
+                                   const uint32_t *trie_of, const uint8_t *trie_flags, const uint8_t *nonzero, int canonical,
+                                   uint32_t *root_trie, uint16_t *root_meta, cudaStream_t st);
 cudaError_t launch_wt_reveal(const DTrieDev &t, const WitnessMarks &w, uint32_t max_list, int canonical, uint32_t *out_trie,
                              uint8_t *out_keys, uint16_t *out_meta, uint32_t *n_out, cudaStream_t st);
-cudaError_t launch_wt_wipe_roots(const DTrieDev &ts, const uint32_t *leaf_of, const uint8_t *trie_flags, uint64_t m, bool write,
-                                 uint32_t *queue, uint32_t *n_queue, uint32_t *n_out, uint32_t *out_trie, uint8_t *out_keys, cudaStream_t st);
-cudaError_t launch_wt_wipe_round(const DTrieDev &ts, uint32_t *queue, uint32_t lo, uint32_t hi, uint32_t *n_queue, uint32_t *n_leaves,
-                                 cudaStream_t st);
-cudaError_t launch_wt_wipe_leaves(const DTrieDev &ts, const uint32_t *queue, uint32_t n, uint32_t *n_out, uint32_t *out_trie,
-                                  uint8_t *out_keys, cudaStream_t st);
+// the wipe queue holds (node, trie) pairs: node | DT_ALT = a node of res
+cudaError_t launch_wt_wipe_roots(const DTrieDev &ts, const DTrieDev &res, const uint32_t *res_trie, const uint32_t *trie_of,
+                                 const uint8_t *trie_flags, uint64_t m, bool write, uint32_t *queue, uint32_t *n_queue, uint32_t *n_out,
+                                 uint32_t *out_trie, uint8_t *out_keys, cudaStream_t st);
+cudaError_t launch_wt_wipe_round(const DTrieDev &ts, const DTrieDev &res, const uint32_t *res_trie, uint32_t *queue, uint32_t lo, uint32_t hi,
+                                 uint32_t *n_queue, uint32_t *n_leaves, cudaStream_t st);
+cudaError_t launch_wt_wipe_leaves(const DTrieDev &ts, const DTrieDev &res, const uint32_t *queue, uint32_t n, uint32_t *n_out,
+                                  uint32_t *out_trie, uint8_t *out_keys, cudaStream_t st);
 cudaError_t launch_wt_clear(const DTrieDev &t, const WitnessMarks &w, const uint32_t *trie_of, const uint8_t *keys, uint64_t n,
                             const uint32_t *leaf_of, uint8_t *trie_flags, cudaStream_t st);
-cudaError_t launch_wt_proof_sizes(const DTrieDev &t, const uint32_t *trie_of, const uint8_t *keys, const uint16_t *meta, uint64_t n_fixed,
-                                  const uint32_t *n_extra, uint64_t n_max, uint32_t *node_count, uint64_t *byte_count, cudaStream_t st);
-cudaError_t launch_wt_proof_write(const DTrieDev &t, const uint32_t *trie_of, const uint8_t *keys, const uint16_t *meta, uint64_t n_fixed,
-                                  const uint32_t *n_extra, uint64_t n_max, const uint64_t *node_base, const uint64_t *byte_base,
-                                  uint64_t node_shift, uint64_t byte_shift, uint8_t *rlp, uint64_t *rlp_offset, cudaStream_t st);
+cudaError_t launch_wt_proof_sizes(const DTrieDev &t, const DTrieDev &res, const uint32_t *res_trie, const uint32_t *trie_of,
+                                  const uint8_t *keys, const uint16_t *meta, uint64_t n_fixed, const uint32_t *n_extra, uint64_t n_max,
+                                  uint32_t *node_count, uint64_t *byte_count, cudaStream_t st);
+cudaError_t launch_wt_proof_write(const DTrieDev &t, const DTrieDev &res, const uint32_t *res_trie, const uint32_t *trie_of,
+                                  const uint8_t *keys, const uint16_t *meta, uint64_t n_fixed, const uint32_t *n_extra, uint64_t n_max,
+                                  const uint64_t *node_base, const uint64_t *byte_base, uint64_t node_shift, uint64_t byte_shift,
+                                  uint8_t *rlp, uint64_t *rlp_offset, cudaStream_t st);
 cudaError_t launch_wt_unique(const uint8_t *sorted32, const uint32_t *perm, const uint64_t *rlp_offset, const uint8_t *rlp, uint64_t n,
                              int drop_empty, uint32_t *keep, uint64_t *kept_bytes, cudaStream_t st);
 cudaError_t launch_wt_gather(const uint8_t *sorted32, const uint32_t *perm, const uint64_t *rlp_offset, const uint8_t *rlp, uint64_t n,
@@ -344,6 +351,7 @@ struct StatelessDev {
     const uint64_t *tseg;        // [n_t + 1] slot targets of account target i
     const uint8_t *tskeys;       // [tseg[n_t]][32]
     uint64_t n_t;
+    int reveal_targets;          // overlay witness: an entry whose key is an account target also reveals its storage without slots
 };
 struct SlNode {  // a queued node: trie, path (packed nibbles, zero-padded) and depth, RLP at rlp[off, off + len)
     uint8_t path[32];

@@ -445,6 +445,29 @@ def witness_batch_arrays(parent_roots, witnesses, blocks) -> tuple:
     return (n, parents, rlp, rlp_off, block_node) + block_batch_arrays(blocks)
 
 
+def _witness_mode(mode: str) -> int:
+    modes = {"legacy": 0, "canonical": 1}
+    if mode not in modes:
+        raise ValueError(f"mode must be one of {sorted(modes)}")
+    return modes[mode]
+
+
+def _witness_block(acct_keys, accounts, flags, slot_keys, values, seg_offsets) -> tuple:
+    """One block in the `apply` layout as contiguous arrays (flags stays None when absent), its sizes checked."""
+    acct_keys = _np(acct_keys).reshape(-1, 32)
+    m = len(acct_keys)
+    accounts = np.ascontiguousarray(accounts, ACCOUNT_DTYPE)
+    fl = None if flags is None else _np(np.asarray(flags, dtype=np.uint8))
+    slot_keys = _np(slot_keys).reshape(-1, 32)
+    values = _np(values).reshape(-1, 32)
+    seg_offsets = _np(seg_offsets, np.uint64)
+    if len(seg_offsets) != m + 1:
+        raise ValueError("seg_offsets must have m+1 entries")
+    if (m and int(seg_offsets[m]) != len(slot_keys)) or len(values) != len(slot_keys):
+        raise ValueError("seg_offsets[m] must equal the number of slot rows (keys and values)")
+    return acct_keys, accounts, fl, slot_keys, values, seg_offsets
+
+
 def block_batch_arrays(blocks) -> tuple:
     """A batch of blocks (`DynamicState.apply` array tuples) concatenated, in ABI order: acct_keys, accts, acct_flags,
     block_acct_offset, slot_keys, values, seg_offsets (b200_witness_roots, b200_dstate_overlay_roots)."""
@@ -990,24 +1013,30 @@ class DynamicState:
                 always_include_root_node: bool = False) -> dict:
         """Execution witness of one block given in the `apply` layout, against the state as it is (the state does not
         change): {keccak(node): node RLP} (TrieWitness::compute; mode "legacy" or "canonical", see include/b200trie.h)."""
-        modes = {"legacy": 0, "canonical": 1}
-        if mode not in modes:
-            raise ValueError(f"mode must be one of {sorted(modes)}")
-        acct_keys = _np(acct_keys).reshape(-1, 32)
-        m = len(acct_keys)
-        accounts = np.ascontiguousarray(accounts, ACCOUNT_DTYPE)
-        fl = None if flags is None else _np(np.asarray(flags, dtype=np.uint8))
-        slot_keys = _np(slot_keys).reshape(-1, 32)
-        values = _np(values).reshape(-1, 32)
-        seg_offsets = _np(seg_offsets, np.uint64)
-        if len(seg_offsets) != m + 1:
-            raise ValueError("seg_offsets must have m+1 entries")
-        if (m and int(seg_offsets[m]) != len(slot_keys)) or len(values) != len(slot_keys):
-            raise ValueError("seg_offsets[m] must equal the number of slot rows (keys and values)")
+        mode_id = _witness_mode(mode)
+        acct_keys, accounts, fl, slot_keys, values, seg_offsets = _witness_block(acct_keys, accounts, flags, slot_keys, values, seg_offsets)
         w = Witness()
         self.engine._check(self.engine.lib.b200_dstate_witness(
-            self.handle, _ptr(acct_keys), _ptr(accounts), _ptr(fl), m, _ptr(slot_keys), _ptr(values), _ptr(seg_offsets),
-            modes[mode], 1 if always_include_root_node else 0, C.byref(w)))
+            self.handle, _ptr(acct_keys), _ptr(accounts), _ptr(fl), len(acct_keys), _ptr(slot_keys), _ptr(values), _ptr(seg_offsets),
+            mode_id, 1 if always_include_root_node else 0, C.byref(w)))
+        return self._witness_map(w)
+
+    def overlay_witness(self, overlay_block, block, mode: str = "legacy", always_include_root_node: bool = False) -> tuple:
+        """b200_dstate_overlay_witness: the witness of `block` on the state after `overlay_block`, against the state as it is
+        (the state does not change; StateProofProvider::witness of a MemoryOverlayStateProvider).  Both are `apply` array
+        tuples (acct_keys, accounts, flags, slot_keys, values, seg_offsets).  -> (overlay root, {keccak(node): node RLP}):
+        exactly what `apply(*overlay_block)` and then `witness(*block, ...)` give on a twin state."""
+        mode_id = _witness_mode(mode)
+        ok, oa, of, osk, osv, oso = _witness_block(*overlay_block)
+        k, a, f, sk, sv, so = _witness_block(*block)
+        root = np.zeros(32, np.uint8)
+        w, s = Witness(), Stats()
+        self.engine._check(self.engine.lib.b200_dstate_overlay_witness(
+            self.handle, _ptr(ok), _ptr(oa), _ptr(of), len(ok), _ptr(osk), _ptr(osv), _ptr(oso), _ptr(k), _ptr(a), _ptr(f), len(k),
+            _ptr(sk), _ptr(sv), _ptr(so), mode_id, 1 if always_include_root_node else 0, _ptr(root), C.byref(w), C.byref(s)))
+        return root.tobytes(), self._witness_map(w)
+
+    def _witness_map(self, w) -> dict:
         try:
             n = int(w.n)
             if not n:

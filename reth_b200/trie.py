@@ -490,6 +490,26 @@ class DynamicStateRoot:
         except Exception as e:  # noqa: BLE001
             raise StateRootError(str(e)) from e
 
+    def overlay_witness(self, input_post, post, mode: str = "legacy", always_include_root_node: bool = False) -> Dict[bytes, bytes]:
+        """StateProofProvider::witness(input, target, mode) of a MemoryOverlayStateProvider (crates/chain-state/src/
+        memory_overlay.rs) in one device call (b200_dstate_overlay_witness): witness(post) on the state after `input_post`,
+        with the state left as it is — debug_executionWitness and the invalid-block witness hook when the parent block is
+        not persisted.  A chain of in-memory blocks is one input_post merged with HashedPostState.extend.  The map is exactly
+        what commit(input_post) and then witness(post, ...) give; `overlay_root(input_post)` is the parent root a stateless
+        client checks it against.  Raises StateRootError for a storage entry of `post` without an account entry
+        (TrieWitnessError::MissingAccount); the layout note of `witness` holds for `post` as well."""
+        for k in post.storages:
+            if k not in post.accounts:
+                raise StateRootError(f"missing account {k.hex()}")
+        _, overlay = self._block(input_post, destroyed_slots=False)
+        _, block = self._block(post, destroyed_slots=True)
+        try:
+            return self.ds.overlay_witness(overlay, block, mode=mode, always_include_root_node=always_include_root_node)[1]
+        except ValueError:
+            raise
+        except Exception as e:  # noqa: BLE001
+            raise StateRootError(str(e)) from e
+
     def overlay_roots(self, posts) -> List[bytes]:
         """StateRootProvider::state_root(hashed_state) on the latest state (crates/storage/storage-api/src/trie.rs) for a batch
         of candidate blocks, in one device call (b200_dstate_overlay_roots): the root `commit` of each post alone would

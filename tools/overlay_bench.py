@@ -27,7 +27,15 @@ updates over a chain of fresh blocks of the same shape.  Each with its time, lau
 --proofs measures the overlay multiproof (b200_dstate_overlay_multiproof) of the first block, alternating rep by rep: with
 the block's accounts and their written slots as targets (what the proof workers ask for); with --touch untouched accounts
 as targets; b200_dstate_multiproof of those untouched targets on the resident state; and b200_dstate_overlay_roots of the
-block.  Each with its time, launches, read-backs and proof node count (account + storage proofs)."""
+block.  Each with its time, launches, read-backs and proof node count (account + storage proofs).
+
+    python tools/overlay_bench.py --witness
+
+--witness measures the overlay witness (b200_dstate_overlay_witness, Legacy): the first block is the overlay, and the target
+is a second block of the same shape on top of it.  Alternating rep by rep: the overlay witness; b200_dstate_overlay_roots of
+the overlay block; b200_dstate_witness of the target block on the resident state.  Each with its time, launches, read-backs
+and node count.  Afterwards the overlay block is applied, and b200_dstate_witness of the target on the changed state must
+give the same map and the overlay root."""
 import argparse
 import ctypes as C
 import json
@@ -55,6 +63,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--updates", action="store_true", help="measure the overlay with TrieUpdates (see above)")
     ap.add_argument("--proofs", action="store_true", help="measure the overlay multiproof (see above)")
+    ap.add_argument("--witness", action="store_true", help="measure the overlay witness (see above)")
     args = ap.parse_args()
     import torch
 
@@ -193,6 +202,50 @@ def main():
         mo = out["overlay_roots"]["device_ms"]["median"]
         out["ratios"] = {k + "_over_overlay_roots": round(out[k]["device_ms"]["median"] / mo, 2)
                          for k in ("overlay_multiproof_block_targets", "overlay_multiproof_untouched", "resident_multiproof_untouched")}
+        out["card_after"] = card()
+        print(json.dumps(out))
+        ds.close()
+        eng.close()
+        return
+
+    if args.witness:
+        a0 = arrays[0]
+        tg = block_arrays(make_block(rng, keys, skeys, offs, args.touch, args.slot_writes))
+        packed = block_batch_arrays(arrays[:1])
+        root, roots = np.zeros(32, np.uint8), np.zeros((1, 32), np.uint8)
+        nodes = {}
+
+        def keep(name, w):
+            nodes[name] = int(w.n)
+            eng.lib.b200_witness_release(C.byref(w))
+
+        def overlay_witness():
+            w = Witness()
+            eng._check(eng.lib.b200_dstate_overlay_witness(ds.handle, *(_ptr(x) for x in a0[:3]), len(a0[0]), *(_ptr(x) for x in a0[3:]),
+                                                           *(_ptr(x) for x in tg[:3]), len(tg[0]), *(_ptr(x) for x in tg[3:]), 0, 0,
+                                                           _ptr(root), C.byref(w), C.byref(Stats())))
+            keep("overlay_witness", w)
+
+        def overlay_root():
+            eng._check(eng.lib.b200_dstate_overlay_roots(ds.handle, 1, *(_ptr(x) for x in packed), _ptr(roots), C.byref(Stats())))
+
+        def resident_witness():
+            w = Witness()
+            eng._check(eng.lib.b200_dstate_witness(ds.handle, *(_ptr(x) for x in tg[:3]), len(tg[0]), *(_ptr(x) for x in tg[3:]), 0, 0,
+                                                   C.byref(w)))
+            keep("resident_witness", w)
+        res = alternating({"overlay_witness": overlay_witness, "overlay_roots": overlay_root, "resident_witness": resident_witness})
+        for k in res:
+            res[k]["witness_nodes"] = nodes.get(k)
+        out.update(res)
+        out["target"] = {"block_accounts": int(len(tg[0])), "block_slot_entries": int(len(tg[3]))}
+        assert root.tobytes() == roots[0].tobytes() and ds.root() == parent
+        ov_root, got = ds.overlay_witness(a0, tg, mode="legacy")
+        assert len(got) == nodes["overlay_witness"] and ov_root == root.tobytes()
+        assert ds.apply(*a0) == ov_root
+        assert got == ds.witness(*tg, mode="legacy"), "overlay witness differs from apply + witness"
+        mo = out["overlay_roots"]["device_ms"]["median"]
+        out["ratios"] = {k + "_over_overlay_roots": round(out[k]["device_ms"]["median"] / mo, 2) for k in ("overlay_witness", "resident_witness")}
         out["card_after"] = card()
         print(json.dumps(out))
         ds.close()
