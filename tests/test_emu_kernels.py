@@ -40,6 +40,21 @@ def test_dynamic_tries_two_stage_rehash_under_cpu_emulation():
     assert " passed" in r.stdout and "failed" not in r.stdout, tail
 
 
+def test_overlay_witness_and_stateless_paths_under_cpu_emulation():
+    """tk_overlay.cuh, tk_witness.cuh and tk_stateless.cuh: the overlay roots, TrieUpdates, multiproofs and witnesses, the
+    execution witness and the stateless roots, and tests/test_gpu_overlay_large.py, whose sizes follow the emulated
+    threshold.  The six random-block cases of 3 000 accounts are left out (about 190 s of the run on an 8-core x86 host,
+    where the rest takes about 8 minutes): test_gpu_overlay_large.py covers those paths at larger sizes."""
+    r = subprocess.run([sys.executable, "-m", "pytest", "tests/test_gpu_overlay.py", "tests/test_gpu_overlay_updates.py",
+                        "tests/test_gpu_overlay_proofs.py", "tests/test_gpu_overlay_witness.py", "tests/test_gpu_witness.py",
+                        "tests/test_gpu_stateless.py", "tests/test_gpu_overlay_large.py", "-m", "gpu", "--emu", "-q", "-x",
+                        "-p", "no:cacheprovider", "-k", "not 3000"],
+                       cwd=ROOT, capture_output=True, text=True, timeout=1500)
+    tail = (r.stdout + r.stderr)[-3000:]
+    assert r.returncode == 0, tail
+    assert " passed" in r.stdout and "failed" not in r.stdout, tail
+
+
 def test_cpp_host_mirror_under_cpu_emulation(tmp_path):
     """tests/cpp/host_test.cpp (reth's trie tests restated over the C++ host mirror) linked against the emulated build."""
     emu = os.path.join(ROOT, "tools", "emu")
