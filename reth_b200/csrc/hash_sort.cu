@@ -309,15 +309,19 @@ __global__ void check_index_kernel(const uint32_t *__restrict__ addr_index, uint
 }  // namespace
 
 // d_ha [n_addr][32], d_hs [n][32] digests; -> d_sorted [n][64], d_perm [n]
+// keys_a / keys_b / idx_a serve both the entries and the nested sort of the address digests, so they are sized for
+// max(n, n_addr) rows before their pointers are taken: the address table may be longer than the batch, and a block the
+// nested sort had to grow would leave ka / kb / ia pointing at freed memory.
 int32_t sort_composite_on_device(b200_ctx *c, const void *d_ha, uint32_t n_addr, const uint32_t *d_addr_index,
                                  const void *d_hs, uint64_t n, void *d_sorted, uint32_t *d_perm, DevBuf &keys_a,
                                  DevBuf &keys_b, DevBuf &idx_a, DevBuf &flag, bool allow_equal) {
     if (n == 0) return B200_OK;
     if (n >= (1ull << 32)) return fail(c, B200_ERR_INVALID_ARG, "at most 2^32-1 entries per sort");
     cudaStream_t st = c->stream;
-    TRY(ensure(c, keys_a, n * 8));
-    TRY(ensure(c, keys_b, n * 8));
-    TRY(ensure(c, idx_a, n * 4));
+    const uint64_t rows = std::max<uint64_t>(n, n_addr);
+    TRY(ensure(c, keys_a, rows * 8));
+    TRY(ensure(c, keys_b, rows * 8));
+    TRY(ensure(c, idx_a, rows * 4));
     TRY(ensure(c, flag, 16));
     uint64_t *ka = static_cast<uint64_t *>(keys_a.p), *kb = static_cast<uint64_t *>(keys_b.p);
     uint32_t *ia = static_cast<uint32_t *>(idx_a.p);

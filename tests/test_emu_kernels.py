@@ -18,7 +18,7 @@ def test_cuda_sources_pass_parity_under_cpu_emulation():
     r = subprocess.run([sys.executable, "-m", "pytest", "tests/test_gpu_trie.py", "tests/test_gpu_keccak.py",
                         "tests/test_gpu_host_mirror.py", "tests/test_gpu_dtrie.py", "tests/test_gpu_dstate.py", "tests/test_gpu_proofs.py",
                         "tests/test_gpu_zz_ordered_roots.py", "tests/test_gpu_zz_table_rows_device.py", "tests/test_gpu_level_classes.py",
-                        "tests/test_gpu_leaf_widths.py", "-m", "gpu", "--emu", "-q", "-x", "-k", FAST,
+                        "tests/test_gpu_leaf_widths.py", "tests/test_gpu_hash_sort_edges.py", "-m", "gpu", "--emu", "-q", "-x", "-k", FAST,
                         "-p", "no:cacheprovider"],
                        cwd=ROOT, capture_output=True, text=True, timeout=1500)
     tail = (r.stdout + r.stderr)[-3000:]
