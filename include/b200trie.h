@@ -717,6 +717,38 @@ B200_API int32_t b200_dstate_overlay_witness(
     const uint8_t *slot_keys32, const uint8_t *values32_be, const uint64_t *seg_offsets /* [m+1] */,
     int32_t mode, int32_t always_include_root,
     uint8_t overlay_root32[32] /* nullable */, b200_witness *out, b200_stats *opt_stats);
+/* Trie changesets of a block: the values its changed trie nodes had before it, against the state as it is, which does not
+ * change (reth: compute_trie_changesets(factory, &trie_updates), crates/trie/trie/src/changesets.rs:50-239, which the payload
+ * validator calls for every block, crates/engine/tree/src/tree/payload_validator.rs:1795, and the changeset cache,
+ * crates/trie/db/src/changesets.rs:69-170; written next to the block, they are applied backwards on unwind).  The input is
+ * the block's TrieUpdatesSorted (crates/trie/common/src/updates.rs:550-556,759-765) reduced to what reth reads of it: paths
+ * and is_deleted.  Paths use the packing of b200_updates (nibbles high-first, zero padded, lengths 1..63) and must be
+ * strictly ascending in reth's Nibbles order, which is the order of (the 32 packed bytes, then the length): a prefix before
+ * its extensions.
+ *   account paths : n_acct_paths of them.
+ *   storage tries : n_storage_tries hashed addresses, strictly ascending; storage_flags[i] bit 0 = is_deleted (nullable: none);
+ *                   trie i's paths are storage_path_offsets[i] .. [i+1] (offsets start at 0, monotone), strictly ascending.
+ * A stored node is a branch whose tree_mask | hash_mask != 0 at a non-empty path: what AccountsTrie / StoragesTrie hold.
+ *   account_out : one record per account path, in input order, trie_id 0: the stored node at exactly that path (seek_exact),
+ *                 or None — all three masks 0 and no hashes, as removed records are.
+ *   storage_out : ordered by trie, then path, trie_id = index into storage_keys32.  A trie that is not deleted: one record per
+ *                 path, as above.  A deleted trie (storage_trie_wiped_changeset_iter, changesets.rs:198-239): the merge by path
+ *                 of its paths with every stored node of the trie — a path the trie holds gives its node, a path it does not
+ *                 gives None, a stored node on no path gives itself.  A key without a resident account, or with an empty
+ *                 storage, has an empty trie: its paths are all None and a deleted one adds nothing.  A trie without records
+ *                 has none in the list (reth leaves an empty storage changeset out); is_deleted is the caller's to copy.
+ * The state is left as it is, so this call comes before the b200_dstate_apply of the block, which overwrites the old nodes.
+ * No paths at all give two valid, empty lists.  Errors: B200_ERR_INVALID_ARG for null pointers with non-zero counts, offsets
+ * that do not start at 0 or are not monotone, a path length of 0 or over 63, non-zero padding, a sharded state, and 2^31-1 or
+ * more records in or out of a list; B200_ERR_UNSORTED for any order violation, duplicates included.  On error both outputs
+ * are released and zeroed.  Release them with b200_updates_release. */
+B200_API int32_t b200_dstate_trie_changesets(
+    b200_dstate *,
+    const uint8_t *acct_path_len, const uint8_t *acct_path_packed /* [n][32] */, uint64_t n_acct_paths,
+    const uint8_t *storage_keys32, const uint8_t *storage_flags /* nullable; bit 0 = is_deleted */, uint64_t n_storage_tries,
+    const uint64_t *storage_path_offsets /* [n_storage_tries+1] */, const uint8_t *storage_path_len,
+    const uint8_t *storage_path_packed /* [N][32] */,
+    b200_updates *account_out, b200_updates *storage_out, b200_stats *opt_stats);
 /* b200_dstate_apply with the block already in device memory (every input pointer and d_root32 are device pointers;
  * n_entries = d_seg_offsets[m]); the update records, if wanted, still arrive in host memory. */
 B200_API int32_t b200_dstate_apply_dev(b200_dstate *, const void *d_acct_keys32, const void *d_accts, const void *d_acct_flags,

@@ -213,6 +213,12 @@ unsafe extern "C" {
                                        acct_flags: *const u8, m: u64, slot_keys32: *const u8, values32_be: *const u8,
                                        seg_offsets: *const u64, mode: i32, always_include_root: i32, overlay_root32: *mut u8,
                                        out: *mut b200_witness, opt_stats: *mut b200_stats) -> i32;
+    /// trie changesets (compute_trie_changesets) of a block's TrieUpdatesSorted paths against the state, which is unchanged
+    pub fn b200_dstate_trie_changesets(state: *mut b200_dstate, acct_path_len: *const u8, acct_path_packed: *const u8,
+                                       n_acct_paths: u64, storage_keys32: *const u8, storage_flags: *const u8,
+                                       n_storage_tries: u64, storage_path_offsets: *const u64, storage_path_len: *const u8,
+                                       storage_path_packed: *const u8, account_out: *mut b200_updates,
+                                       storage_out: *mut b200_updates, opt_stats: *mut b200_stats) -> i32;
     pub fn b200_witness_release(w: *mut b200_witness);
     /// CPUs + preferred memory of the calling thread on the GPU's NUMA node (before allocating staging buffers)
     pub fn b200_numa_bind_thread(device_ordinal: i32) -> i32;

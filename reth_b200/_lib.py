@@ -234,6 +234,7 @@ def load():
         C.POINTER(Proofs), PS)
     sig("b200_dstate_overlay_witness", i32, vp, vp, vp, vp, u64, vp, vp, vp, vp, vp, vp, u64, vp, vp, vp, i32, i32, vp,
         C.POINTER(Witness), PS)
+    sig("b200_dstate_trie_changesets", i32, vp, vp, vp, u64, vp, vp, u64, vp, vp, vp, PU, PU, PS)
     sig("b200_dstate_apply_dev", i32, vp, vp, vp, vp, u64, vp, vp, vp, u64, vp, PU, PU, PU, PU, vp, PS)
     sig("b200_dstate_root", i32, vp, vp)
     sig("b200_dstate_accounts", u64, vp)

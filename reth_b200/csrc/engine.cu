@@ -379,6 +379,7 @@ extern "C" B200_API uint64_t b200_launch_count(const b200_ctx *c) { return c ? c
 #include "eng_dstate.inl"
 #include "eng_proofs.inl"
 #include "eng_witness.inl"
+#include "eng_changesets.inl"
 #include "eng_ordered.inl"
 #include "eng_items.inl"
 #include "eng_stateless.inl"

@@ -139,15 +139,20 @@ __global__ void dt_recycle_kernel(DTrieDev t) {  // end of an apply: this apply'
     if (i >= t.g[DG_FREED_NOW]) return;
     t.node_free[t.g[DG_NODE_FREE] + i] = t.freed_now[i];
 }
+// byte b of the first d nibbles of key, packed high-first and zero padded (the path layout of b200_updates)
+static __device__ __forceinline__ uint8_t dt_path_byte(const uint8_t *key, uint32_t d, uint32_t b) {
+    return (uint8_t)(2 * b + 1 < d ? key[b] : (2 * b < d ? (key[b] & 0xF0) : 0));
+}
+static __device__ __forceinline__ void dt_pack_path(const uint8_t *key, uint32_t d, uint8_t *pp) {
+    for (uint32_t b = 0; b < 32; b++) pp[b] = dt_path_byte(key, d, b);
+}
 __global__ void dt_removed_paths_kernel(DTrieDev t, uint32_t n_removed, uint8_t *__restrict__ path_len, uint8_t *__restrict__ path_packed,
                                         uint32_t *__restrict__ trie_id) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n_removed) return;
     uint32_t v = t.removed[i];
     uint32_t d = t.nmasks[v].w;
-    const uint8_t *key = t.nkey + 32 * (uint64_t)v;
-    uint8_t *pp = path_packed + 32 * (uint64_t)i;
-    for (uint32_t b = 0; b < 32; b++) pp[b] = (uint8_t)(2 * b + 1 < d ? key[b] : (2 * b < d ? (key[b] & 0xF0) : 0));
+    dt_pack_path(t.nkey + 32 * (uint64_t)v, d, path_packed + 32 * (uint64_t)i);
     path_len[i] = (uint8_t)d;
     trie_id[i] = t.ntrie ? t.ntrie[v] : 0;
 }
@@ -998,22 +1003,16 @@ __global__ void dt_stored_flags_kernel(DTrieDev t, const uint32_t *__restrict__ 
     flags[i] = stored ? 1 : 0;
     n_hashes[i] = stored ? (uint32_t)__popc(t.nmasks[v].z) : 0u;
 }
-__global__ void dt_gather_updates_kernel(DTrieDev t, const uint32_t *__restrict__ stored_ids, uint32_t n_stored,
-                                         const uint32_t *__restrict__ hash_prefix_by_record, UpdatesDev out) {
-    uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n_stored) return;
-    uint32_t v = stored_ids[i];
-    ushort4 m = t.nmasks[v];
-    uint32_t d = m.w;
-    out.trie_id[i] = t.ntrie ? t.ntrie[v] : 0;
-    out.path_len[i] = (uint8_t)d;
-    const uint8_t *key = t.nkey + 32 * (uint64_t)v;
-    uint8_t *pp = out.path_packed + 32 * (uint64_t)i;
-    for (uint32_t b = 0; b < 32; b++) pp[b] = (uint8_t)(2 * b + 1 < d ? key[b] : (2 * b < d ? (key[b] & 0xF0) : 0));
+// record i of `out`: stored node v as a BranchNodeCompact of trie trie_id, its child hashes from hash slot h on
+static __device__ __forceinline__ void dt_put_record(const DTrieDev &t, uint32_t v, uint32_t trie_id, uint32_t h, const UpdatesDev &out,
+                                                     uint32_t i) {
+    const ushort4 m = t.nmasks[v];
+    out.trie_id[i] = trie_id;
+    out.path_len[i] = (uint8_t)m.w;
+    dt_pack_path(t.nkey + 32 * (uint64_t)v, m.w, out.path_packed + 32 * (uint64_t)i);
     out.state_mask[i] = m.x;
     out.tree_mask[i] = m.y;
     out.hash_mask[i] = m.z;
-    uint32_t h = hash_prefix_by_record[i];
     out.hash_offset[i] = h;
     const uint32_t *ch = t.nchild + 16 * (uint64_t)v;
     for (int s = 0; s < 16; s++)
@@ -1021,5 +1020,12 @@ __global__ void dt_gather_updates_kernel(DTrieDev t, const uint32_t *__restrict_
             dt_copy32(out.hashes + 32 * (uint64_t)h, t.nref + 32 * (uint64_t)ch[s]);
             h++;
         }
+}
+__global__ void dt_gather_updates_kernel(DTrieDev t, const uint32_t *__restrict__ stored_ids, uint32_t n_stored,
+                                         const uint32_t *__restrict__ hash_prefix_by_record, UpdatesDev out) {
+    uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_stored) return;
+    const uint32_t v = stored_ids[i];
+    dt_put_record(t, v, t.ntrie ? t.ntrie[v] : 0, hash_prefix_by_record[i], out, i);
 }
 

@@ -278,7 +278,8 @@ static __device__ void wt_wipe_child(const DTrieDev &ts, const DTrieDev &res, co
         wt_wipe_push(queue, n_queue, w | alt, trie);
     }
 }
-// roots: a leaf root is counted (WRITE: written as a target); a node root is queued (count pass only)
+// roots: a leaf root is counted (WRITE: written as a target); a node root is queued (count pass only).  trie_flags nullable:
+// every trie of trie_of is expanded (DT_NONE: none).
 template <bool WRITE>
 __global__ void wt_wipe_roots_kernel(DTrieDev ts, DTrieDev res, const uint32_t *__restrict__ res_trie, const uint32_t *__restrict__ trie_of,
                                      const uint8_t *__restrict__ trie_flags, uint64_t m, uint32_t *__restrict__ queue,
@@ -287,7 +288,7 @@ __global__ void wt_wipe_roots_kernel(DTrieDev ts, DTrieDev res, const uint32_t *
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= m) return;
     const uint32_t trie = trie_of[i];
-    if (trie == DT_NONE || !(trie_flags[trie] & WF_WIPED)) return;
+    if (trie == DT_NONE || (trie_flags && !(trie_flags[trie] & WF_WIPED))) return;
     const uint32_t w = ts.troot[trie];
     if (!WRITE) {
         wt_wipe_child(ts, res, res_trie, w, trie, 0u, queue, n_queue, n_out);

@@ -39,6 +39,7 @@ namespace b200 {
 #include "tk_proofs.cuh"
 #include "tk_dtrie_launchers.cuh"
 #include "tk_witness.cuh"
+#include "tk_changesets.cuh"
 #include "tk_stateless.cuh"
 #include "tk_overlay.cuh"
 

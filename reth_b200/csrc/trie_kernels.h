@@ -302,7 +302,7 @@ cudaError_t launch_wt_account_walk(const DTrieDev &ta, const DTrieDev &ts, const
                                    uint32_t *root_trie, uint16_t *root_meta, cudaStream_t st);
 cudaError_t launch_wt_reveal(const DTrieDev &t, const WitnessMarks &w, uint32_t max_list, int canonical, uint32_t *out_trie,
                              uint8_t *out_keys, uint16_t *out_meta, uint32_t *n_out, cudaStream_t st);
-// the wipe queue holds (node, trie) pairs: node | DT_ALT = a node of res
+// the wipe queue holds (node, trie) pairs: node | DT_ALT = a node of res; trie_flags nullable: every trie of trie_of is wiped
 cudaError_t launch_wt_wipe_roots(const DTrieDev &ts, const DTrieDev &res, const uint32_t *res_trie, const uint32_t *trie_of,
                                  const uint8_t *trie_flags, uint64_t m, bool write, uint32_t *queue, uint32_t *n_queue, uint32_t *n_out,
                                  uint32_t *out_trie, uint8_t *out_keys, cudaStream_t st);
@@ -324,6 +324,20 @@ cudaError_t launch_wt_unique(const uint8_t *sorted32, const uint32_t *perm, cons
 cudaError_t launch_wt_gather(const uint8_t *sorted32, const uint32_t *perm, const uint64_t *rlp_offset, const uint8_t *rlp, uint64_t n,
                              const uint32_t *keep, const uint32_t *pos, const uint64_t *byte_pos, uint8_t *out_hash, uint64_t *out_offset,
                              uint8_t *out_rlp, cudaStream_t st);
+
+// ------------------------------------------------------------------------------------------------ trie changesets (tk_changesets.cuh)
+// a row is (output trie id << 32 | source): a changed-path index, or CS_NODE | a node id of a deleted trie
+cudaError_t launch_cs_lookup(const DTrieDev &t, const uint64_t *offs, uint64_t n_keys, const uint32_t *leaf_of, const uint8_t *kflags,
+                             const uint8_t *len, const uint8_t *paths, uint64_t n, uint32_t *node_of, uint64_t *rows, uint32_t *n_rows,
+                             cudaStream_t st);
+cudaError_t launch_cs_wiped_rows(const DTrieDev &ts, const DTrieDev &ta, const uint32_t *queue, uint32_t n_queue, const uint8_t *keys32,
+                                 uint64_t n_keys, uint64_t *rows, uint32_t *n_rows, cudaStream_t st);
+cudaError_t launch_cs_sort_word(const DTrieDev &t, const uint8_t *len, const uint8_t *paths, const uint64_t *rows, uint32_t n, int w,
+                                uint64_t *keys64, cudaStream_t st);
+cudaError_t launch_cs_hash_counts(const DTrieDev &t, const uint64_t *rows, uint32_t n, const uint32_t *node_of, uint32_t *n_hashes,
+                                  cudaStream_t st);
+cudaError_t launch_cs_write(const DTrieDev &t, const uint64_t *rows, uint32_t n, const uint32_t *node_of, const uint8_t *len,
+                            const uint8_t *paths, const uint32_t *hash_prefix, const UpdatesDev &out, cudaStream_t st);
 
 // ------------------------------------------------------------------------------------------------ stateless roots (tk_stateless.cuh)
 enum : uint32_t { SL_INCOMPLETE = 1u, SL_INVALID = 2u, SL_NONE = 0xFFFFFFFFu };

@@ -39,6 +39,17 @@ def _unpack_nibbles(packed: bytes, n: int) -> bytes:
     return bytes(x for b in packed for x in (b >> 4, b & 15))[:n]
 
 
+def _pack_paths(paths) -> tuple:
+    """nibble paths -> (lengths u8[n], [n][32] packed high-first, zero padded): the path layout of b200_updates"""
+    n = len(paths)
+    lens = np.array([len(p) for p in paths], np.uint8)
+    packed = np.zeros((n, 32), np.uint8)
+    for i, p in enumerate(paths):
+        nib = bytes(p) + b"\0" * (len(p) & 1)
+        packed[i, :len(nib) // 2] = np.frombuffer(bytes(nib[k] << 4 | nib[k + 1] for k in range(0, len(nib), 2)), np.uint8)
+    return lens, packed
+
+
 def updates_to_records(u: Updates, lib, sort: bool = True) -> list:
     """-> [(trie_id, path_nibbles, state_mask, tree_mask, hash_mask, [hashes])] sorted by (trie_id, path);
     releases the library-owned buffers.  (sort=False keeps the library's order: full builds already deliver table
@@ -1077,6 +1088,30 @@ class DynamicState:
                         [(r[0] - lo,) + r[1:] for r in su if lo <= r[0] < hi], [(r[0] - lo, r[1]) for r in sr if lo <= r[0] < hi],
                         deleted[lo:hi].copy()))
         return out
+
+    def trie_changesets(self, acct_paths, storage: dict) -> tuple:
+        """b200_dstate_trie_changesets: the values the changed trie nodes of a block had before it, against the state as it
+        is (the state does not change; reth's compute_trie_changesets).  acct_paths: the block's changed account-trie paths
+        (nibble strings), sorted; storage: {hashed address: (is_deleted, sorted changed paths)}.  -> (account records,
+        storage records), records shaped as `apply(..., want_updates=True)` returns them: (trie_id, path, state_mask,
+        tree_mask, hash_mask, [hashes]), all masks 0 and no hashes for None; a storage record's trie_id is the index of its
+        address in sorted(storage).  Order: account records in input order; storage records by trie, then path."""
+        alen, apk = _pack_paths(acct_paths)
+        addrs = sorted(storage)
+        n = len(addrs)
+        keys = np.frombuffer(b"".join(addrs), np.uint8).reshape(n, 32) if n else np.zeros((0, 32), np.uint8)
+        flags = np.array([1 if storage[a][0] else 0 for a in addrs], np.uint8)
+        paths, offs = [], [0]
+        for a in addrs:
+            paths.extend(storage[a][1])
+            offs.append(len(paths))
+        slen, spk = _pack_paths(paths)
+        offs = np.array(offs, np.uint64)
+        au, su, s = Updates(), Updates(), Stats()
+        lib = self.engine.lib
+        self.engine._check(lib.b200_dstate_trie_changesets(self.handle, _ptr(alen), _ptr(apk), len(alen), _ptr(keys), _ptr(flags), n,
+                                                           _ptr(offs), _ptr(slen), _ptr(spk), C.byref(au), C.byref(su), C.byref(s)))
+        return updates_to_records(au, lib, sort=False), updates_to_records(su, lib, sort=False)
 
     def account_proofs(self, acct_keys) -> list:
         """-> for every target hashed address the list of node RLPs from the root down (Proof::account_proof)."""

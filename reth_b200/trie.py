@@ -48,6 +48,31 @@ class StorageTrieUpdates:
     def __len__(self):
         return int(self.is_deleted) + len(self.storage_nodes) + len(self.removed_nodes)
 
+    def into_sorted(self) -> "StorageTrieUpdatesSorted":
+        """updates.rs:364-379: updated nodes, then the removed paths that are not updated as None, sorted by path."""
+        nodes = [(p, n) for p, n in self.storage_nodes.items()]
+        nodes += [(p, None) for p in self.removed_nodes if p not in self.storage_nodes]
+        nodes.sort(key=lambda e: e[0])
+        return StorageTrieUpdatesSorted(self.is_deleted, nodes)
+
+
+@dataclass
+class StorageTrieUpdatesSorted:
+    """crates/trie/common/src/updates.rs:759-765: (path, Some(node) | None) sorted by path."""
+    is_deleted: bool = False
+    storage_nodes: List[Tuple[Nibbles, Optional[BranchNodeCompact]]] = field(default_factory=list)
+
+    def is_empty(self) -> bool:
+        return not self.is_deleted and not self.storage_nodes
+
+
+@dataclass
+class TrieUpdatesSorted:
+    """crates/trie/common/src/updates.rs:550-556: account (path, Some(node) | None) sorted by path, and the sorted updates
+    of every storage trie by hashed address."""
+    account_nodes: List[Tuple[Nibbles, Optional[BranchNodeCompact]]] = field(default_factory=list)
+    storage_tries: Dict[B256, StorageTrieUpdatesSorted] = field(default_factory=dict)
+
 
 @dataclass
 class TrieUpdates:
@@ -64,6 +89,13 @@ class TrieUpdates:
 
     def is_empty(self) -> bool:
         return not self.account_nodes and not self.removed_nodes and not self.storage_tries
+
+    def into_sorted(self) -> TrieUpdatesSorted:
+        """updates.rs:160-180: updated takes precedence over removed, then every list is sorted by path."""
+        nodes = [(p, n) for p, n in self.account_nodes.items()]
+        nodes += [(p, None) for p in self.removed_nodes if p not in self.account_nodes]
+        nodes.sort(key=lambda e: e[0])
+        return TrieUpdatesSorted(nodes, {k: v.into_sorted() for k, v in self.storage_tries.items()})
 
 
 @dataclass
@@ -548,6 +580,39 @@ class DynamicStateRoot:
             raise
         except Exception as e:  # noqa: BLE001
             raise StateRootError(str(e)) from e
+
+    def trie_changesets(self, updates) -> TrieUpdatesSorted:
+        """compute_trie_changesets(factory, &trie_updates) (crates/trie/trie/src/changesets.rs:50-239) with this state as the
+        trie cursor factory, in one device call (b200_dstate_trie_changesets): the values the nodes a block changes had before
+        it, which reth writes next to the block and applies backwards on unwind.  updates: the block's TrieUpdatesSorted (a
+        TrieUpdates is sorted first); only its paths and is_deleted are read.  -> TrieUpdatesSorted of the old values: each
+        account path, and each path of a storage trie that is not deleted, with the node stored at exactly that path or None;
+        a deleted storage trie gets every node it stored merged in by path (storage_trie_wiped_changeset_iter); storage tries
+        with an empty changeset are left out.  The state does not change.
+
+        On the live path the order is overlay_root_with_updates(post) -> trie_changesets(updates) -> commit(post): the call
+        reads the nodes as they are before the block, and the commit overwrites them.  The parent is the resident state itself;
+        changesets against a parent that is an unpersisted overlay (reth's InMemoryTrieCursorFactory over cumulative updates)
+        are not covered."""
+        if isinstance(updates, TrieUpdates):
+            updates = updates.into_sorted()
+        addrs = sorted(updates.storage_tries)
+        storage = {a: (updates.storage_tries[a].is_deleted, [p for p, _ in updates.storage_tries[a].storage_nodes]) for a in addrs}
+        try:
+            acct, stor = self.ds.trie_changesets([p for p, _ in updates.account_nodes], storage)
+        except ValueError:
+            raise
+        except Exception as e:  # noqa: BLE001
+            raise StateRootError(str(e)) from e
+        node = lambda r: BranchNodeCompact(r[2], r[3], r[4], tuple(r[5])) if r[2] else None  # state_mask 0: None
+        out = TrieUpdatesSorted([(r[1], node(r)) for r in acct])
+        per_trie: Dict[int, list] = {}
+        for r in stor:
+            per_trie.setdefault(r[0], []).append((r[1], node(r)))
+        for i, a in enumerate(addrs):
+            if per_trie.get(i):
+                out.storage_tries[a] = StorageTrieUpdatesSorted(updates.storage_tries[a].is_deleted, per_trie[i])
+        return out
 
     def _overlay(self, posts, want_updates: bool):
         layouts = [self._block(post, destroyed_slots=False) for post in posts]
