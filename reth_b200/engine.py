@@ -463,7 +463,7 @@ def _witness_mode(mode: str) -> int:
     return modes[mode]
 
 
-def _witness_block(acct_keys, accounts, flags, slot_keys, values, seg_offsets) -> tuple:
+def _block_args(acct_keys, accounts, flags, slot_keys, values, seg_offsets) -> tuple:
     """One block in the `apply` layout as contiguous arrays (flags stays None when absent), its sizes checked."""
     acct_keys = _np(acct_keys).reshape(-1, 32)
     m = len(acct_keys)
@@ -483,16 +483,14 @@ def block_batch_arrays(blocks) -> tuple:
     """A batch of blocks (`DynamicState.apply` array tuples) concatenated, in ABI order: acct_keys, accts, acct_flags,
     block_acct_offset, slot_keys, values, seg_offsets (b200_witness_roots, b200_dstate_overlay_roots)."""
     keys, accts, flags, skeys, svals, offs, block_acct = [], [], [], [], [], [0], [0]
-    for k, a, f, sk, sv, so in blocks:
-        k = _np(k).reshape(-1, 32)
+    for block in blocks:
+        k, a, f, sk, sv, so = _block_args(*block)
         m = len(k)
-        so = _np(so, np.uint64)
-        sk, sv = _np(sk).reshape(-1, 32), _np(sv).reshape(-1, 32)
-        if len(so) != m + 1 or int(so[0]) != 0 or int(so[m]) != len(sk) or len(sv) != len(sk):
-            raise ValueError("seg_offsets must have m+1 entries from 0 to the number of slot rows (keys and values)")
+        if int(so[0]) != 0 or int(so[m]) != len(sk):
+            raise ValueError("seg_offsets must run from 0 to the number of slot rows")
         keys.append(k)
-        accts.append(np.ascontiguousarray(a, ACCOUNT_DTYPE).reshape(m))
-        flags.append(np.ones(m, np.uint8) if f is None else _np(np.asarray(f, dtype=np.uint8)).reshape(m))
+        accts.append(a.reshape(m))
+        flags.append(np.ones(m, np.uint8) if f is None else f.reshape(m))
         skeys.append(sk)
         svals.append(sv)
         offs.extend((so[1:] + np.uint64(offs[-1])).tolist())
@@ -880,17 +878,8 @@ class DynamicState:
     def apply(self, acct_keys, accounts, flags, slot_keys, values, seg_offsets, want_updates=False):
         """-> root, or (root, acct_updated, acct_removed_paths, storage_updated, storage_removed [(entry, path)],
         storage_deleted flags) with want_updates."""
-        acct_keys = _np(acct_keys).reshape(-1, 32)
+        acct_keys, accounts, fl, slot_keys, values, seg_offsets = _block_args(acct_keys, accounts, flags, slot_keys, values, seg_offsets)
         m = len(acct_keys)
-        accounts = np.ascontiguousarray(accounts, ACCOUNT_DTYPE)
-        fl = None if flags is None else _np(np.asarray(flags, dtype=np.uint8))
-        slot_keys = _np(slot_keys).reshape(-1, 32)
-        values = _np(values).reshape(-1, 32)
-        seg_offsets = _np(seg_offsets, np.uint64)
-        if len(seg_offsets) != m + 1:
-            raise ValueError("seg_offsets must have m+1 entries")
-        if (m and int(seg_offsets[m]) != len(slot_keys)) or len(values) != len(slot_keys):
-            raise ValueError("seg_offsets[m] must equal the number of slot rows (keys and values)")
         root = np.empty(32, np.uint8)
         au, ar, su, sr, s = Updates(), Updates(), Updates(), Updates(), Stats()
         deleted = np.zeros(max(m, 1), np.uint8)
@@ -1025,7 +1014,7 @@ class DynamicState:
         """Execution witness of one block given in the `apply` layout, against the state as it is (the state does not
         change): {keccak(node): node RLP} (TrieWitness::compute; mode "legacy" or "canonical", see include/b200trie.h)."""
         mode_id = _witness_mode(mode)
-        acct_keys, accounts, fl, slot_keys, values, seg_offsets = _witness_block(acct_keys, accounts, flags, slot_keys, values, seg_offsets)
+        acct_keys, accounts, fl, slot_keys, values, seg_offsets = _block_args(acct_keys, accounts, flags, slot_keys, values, seg_offsets)
         w = Witness()
         self.engine._check(self.engine.lib.b200_dstate_witness(
             self.handle, _ptr(acct_keys), _ptr(accounts), _ptr(fl), len(acct_keys), _ptr(slot_keys), _ptr(values), _ptr(seg_offsets),
@@ -1038,8 +1027,8 @@ class DynamicState:
         tuples (acct_keys, accounts, flags, slot_keys, values, seg_offsets).  -> (overlay root, {keccak(node): node RLP}):
         exactly what `apply(*overlay_block)` and then `witness(*block, ...)` give on a twin state."""
         mode_id = _witness_mode(mode)
-        ok, oa, of, osk, osv, oso = _witness_block(*overlay_block)
-        k, a, f, sk, sv, so = _witness_block(*block)
+        ok, oa, of, osk, osv, oso = _block_args(*overlay_block)
+        k, a, f, sk, sv, so = _block_args(*block)
         root = np.zeros(32, np.uint8)
         w, s = Witness(), Stats()
         self.engine._check(self.engine.lib.b200_dstate_overlay_witness(
