@@ -526,6 +526,19 @@ B200_API int32_t b200_dstate_create_dev(b200_ctx *, const void *d_acct_keys32, c
                                         const void *d_slot_keys32, const void *d_values32_be, const void *d_seg_offsets,
                                         uint64_t n_slots, int32_t sharded, b200_dstate **out, void *d_root32 /* nullable */);
 B200_API int32_t b200_dstate_frontier(b200_dstate *, b200_frontier_entry out16[16]);
+/* The frontier entries of a sharded state after each of a batch of candidate blocks, each applied on its own to the state
+ * as it is (siblings, not a chain); the state does not change.  The ranks all-gather out (n_blocks x 16 x 68 bytes) and
+ * b200_root_from_frontier of block b's merged entries is the root b200_dstate_overlay_roots gives on an unsharded state:
+ * payload validation and payload building over a sharded state, before b200_dstate_apply keeps one block.  Inputs in the
+ * layout and with the rules of b200_dstate_overlay_roots (each rank passes its part of every block).  out[16b .. 16b + 15]
+ * = what b200_dstate_frontier returns after b200_dstate_apply of block b alone: a bucket the block does not touch keeps its
+ * entry, a bucket it empties gives an all-zero entry.  A block without entries gives the current frontier.  Errors:
+ * B200_ERR_INVALID_ARG for an unsharded state and as b200_dstate_overlay_roots (null pointers, bad offsets, the limits),
+ * B200_ERR_UNSORTED; out is zeroed on any error. */
+B200_API int32_t b200_dstate_overlay_frontiers(b200_dstate *, uint64_t n_blocks, const uint8_t *acct_keys32, const b200_account *accts,
+                                               const uint8_t *acct_flags /* nullable */, const uint64_t *block_acct_offset /* [n_blocks+1] */,
+                                               const uint8_t *slot_keys32, const uint8_t *values32_be, const uint64_t *seg_offsets /* [M+1] */,
+                                               b200_frontier_entry *out /* [n_blocks][16] */, b200_stats *opt_stats);
 /* Merkle proofs from the resident state (SURVEY.md §8 f4; eth_getProof / reth's Proof::account_proof and storage_proof,
  * crates/trie/trie/src/proof/mod.rs): target t's proof is nodes node_offset[t] .. node_offset[t+1], node k's RLP is
  * rlp[rlp_offset[k] .. rlp_offset[k+1]), root first — every node whose position is a prefix of the target key (what

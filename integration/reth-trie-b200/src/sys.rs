@@ -158,6 +158,12 @@ unsafe extern "C" {
                              storage_updated: *mut b200_updates, storage_removed: *mut b200_updates,
                              storage_deleted: *mut u8, stats: *mut b200_stats) -> i32;
     pub fn b200_dstate_frontier(state: *mut b200_dstate, out16: *mut b200_frontier_entry) -> i32;
+    /// the frontier entries of a sharded state after each sibling block (out: [n_blocks][16]), the state unchanged; the ranks
+    /// all-gather them and b200_root_from_frontier gives each block's root (payload validation over a sharded state)
+    pub fn b200_dstate_overlay_frontiers(state: *mut b200_dstate, n_blocks: u64, acct_keys32: *const u8, accts: *const b200_account,
+                                         acct_flags: *const u8, block_acct_offset: *const u64, slot_keys32: *const u8,
+                                         values32_be: *const u8, seg_offsets: *const u64, out: *mut b200_frontier_entry,
+                                         stats: *mut b200_stats) -> i32;
     pub fn b200_root_from_frontier(ctx: *mut b200_ctx, frontier16: *const b200_frontier_entry, root32: *mut u8) -> i32;
     pub fn b200_dstate_destroy(state: *mut b200_dstate);
     /// transactions / receipts / withdrawals roots of a batch of lists (ordered_root.rs:240-257 per list)

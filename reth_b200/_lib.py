@@ -229,6 +229,7 @@ def load():
     sig("b200_witness_release", None, C.POINTER(Witness))
     sig("b200_witness_roots", i32, vp, u64, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, PS)
     sig("b200_dstate_overlay_roots", i32, vp, u64, vp, vp, vp, vp, vp, vp, vp, vp, PS)
+    sig("b200_dstate_overlay_frontiers", i32, vp, u64, vp, vp, vp, vp, vp, vp, vp, C.POINTER(FrontierEntry), PS)
     sig("b200_dstate_overlay_roots_with_updates", i32, vp, u64, vp, vp, vp, vp, vp, vp, vp, vp, PU, PU, PU, PU, vp, PS)
     sig("b200_dstate_overlay_multiproof", i32, vp, vp, vp, vp, u64, vp, vp, vp, vp, u64, vp, vp, vp, C.POINTER(Proofs), vp,
         C.POINTER(Proofs), PS)

@@ -89,7 +89,7 @@ struct b200_ctx {
     DevBuf sort_aux[4];  // composite sort: sorted address digests, their permutation, head flags / dense ranks, rank by address
     DevBuf node_key, node_key2, node_ids, node_order;
     DevBuf ord_keys, ord_knib, ord_item, ord_sched, ord_sched2, ord_pos, ord_order;  // ordered tries (eng_ordered.inl)
-    DevBuf sl[28];  // stateless roots (eng_stateless.inl) and overlay roots (eng_overlay.inl)
+    DevBuf sl[29];  // stateless roots (eng_stateless.inl) and overlay roots (eng_overlay.inl)
     // staging for host-pointer entry points
     DevBuf in_a, in_b, in_c, in_d, in_e, out_a, chunk_in[3], chunk_out[3];
     void *pinned_small = nullptr;  // 4 KiB page-locked readback area

@@ -3,10 +3,54 @@
 // files use the device functions of the earlier ones).
 
 // ------------------------------------------------------------------------------------------------ multi-GPU frontier
+// The frontier entry of a trie of forest f whose keys share their first nibble, from its top item (f.S of its first leaf):
+// as_root is the trie's root (the item's reference as the top of its trie, which is always hashed), as_child re-encodes
+// only the top node with parent depth 0.  The item is a leaf, a branch node (f.n + node id), or, when `nibs` is given (an
+// items fold), possibly a hash item of depth L = nibs[item] < 64: the hash of an unrevealed branch at depth L, whose
+// reference from depth 0 is that hash, wrapped in an extension over nibbles 1 .. L-1 when L > 1.
+template <int BLOCK, bool ACCOUNT, bool ITEMS>
+__device__ __forceinline__ void frontier_entry(Strip<BLOCK> &s, const ForestDev &f, uint32_t item, const uint8_t *__restrict__ values,
+                                               const uint8_t *__restrict__ storage_roots, const uint8_t *__restrict__ nibs,
+                                               FrontierEntryDev &e) {
+    uint32_t ref[8], hashed = 0, exts = 0, meta;
+    const uint8_t *rootp =
+        item < f.n ? f.leaf_ref + 32 * (uint64_t)item : f.node_ref + 32 * (uint64_t)(item - (uint32_t)f.n);
+    load32_nc(rootp, ref);
+    e.as_root_len = 32;
+    for (int i = 0; i < 32; i++) e.as_root[i] = (uint8_t)(ref[i >> 2] >> (8 * (i & 3)));
+    const uint32_t stride = ACCOUNT ? (uint32_t)sizeof(b200_account_dev) : 32u;
+    if (ITEMS && item < f.n && nibs[item] < 64) {
+        const uint2 *q = reinterpret_cast<const uint2 *>(values + (uint64_t)stride * item);  // rows are 8-byte aligned
+        for (int w = 0; w < 4; w++) {
+            const uint2 t = __ldg(q + w);
+            ref[2 * w] = t.x;
+            ref[2 * w + 1] = t.y;
+        }
+        meta = thread_finish_node(s, ref, 0u, 0, (int)nibs[item], f.keys + 32 * (uint64_t)item, hashed, exts);
+    } else if (item < f.n) {
+        uint32_t k[8];
+        load32(f.keys + 32 * (uint64_t)item, k);
+        const uint8_t *vp = values + (uint64_t)stride * item;
+        const uint8_t *sp = (ACCOUNT && storage_roots) ? storage_roots + 32 * (uint64_t)item : nullptr;
+        uint32_t len = encode_leaf<Strip<BLOCK>, ACCOUNT>(s, k, 0, vp, sp, f.err);
+        meta = strip_to_ref(s, len, false, ref, hashed);
+    } else {
+        uint32_t v = item - (uint32_t)f.n;
+        uint32_t d = f.node_masks[v].w;
+        uint32_t j0 = f.node_start[v], k = f.node_start[v + 1] - j0;
+        uint32_t sm, tm, hm, l, r;
+        uint32_t len = encode_branch_u<BLOCK, 16>(s, f, j0, k, sm, tm, hm, l, r);
+        meta = strip_to_ref(s, len, false, ref, hashed);
+        meta = thread_finish_node(s, ref, meta, 0, (int)d, f.keys + 32 * (uint64_t)l, hashed, exts);
+    }
+    LinBuf lb{e.as_child, 0};
+    put_child(lb, ref, meta & META_LEN);
+    e.as_child_len = (uint8_t)lb.n;
+}
+
 // For each of the 16 top-nibble buckets of this rank's account shard: the bucket's node as child of a depth-0
 // root branch (as_child) and as a trie of its own (as_root).  The build treated every bucket as a separate
-// trie (boundary gaps), so as_root is simply the segment root; as_child re-encodes only the bucket's top node
-// with parent depth 0.
+// trie (boundary gaps), so as_root is simply the segment root.
 template <int BLOCK, bool ACCOUNT>
 __global__ void frontier_kernel(ForestDev f, const uint64_t *__restrict__ bucket_offsets /*17*/,
                                 const uint8_t *__restrict__ values, const uint8_t *__restrict__ storage_roots,
@@ -20,34 +64,7 @@ __global__ void frontier_kernel(ForestDev f, const uint64_t *__restrict__ bucket
     for (int i = 0; i < 33; i++) e.as_child[i] = e.as_root[i] = 0;
     e.as_child_len = e.as_root_len = 0;
     uint64_t lo = bucket_offsets[b], hi = bucket_offsets[b + 1];
-    if (lo < hi) {
-        uint32_t item = f.S[lo];
-        uint32_t ref[8], hashed = 0, exts = 0, meta;
-        const uint8_t *rootp =
-            item < f.n ? f.leaf_ref + 32 * (uint64_t)item : f.node_ref + 32 * (uint64_t)(item - (uint32_t)f.n);
-        load32_nc(rootp, ref);
-        e.as_root_len = 32;
-        for (int i = 0; i < 32; i++) e.as_root[i] = (uint8_t)(ref[i >> 2] >> (8 * (i & 3)));
-        if (item < f.n) {
-            uint32_t k[8];
-            load32(f.keys + 32 * (uint64_t)item, k);
-            const uint8_t *vp = ACCOUNT ? values + (uint64_t)sizeof(b200_account_dev) * item : values + 32 * (uint64_t)item;
-            const uint8_t *sp = (ACCOUNT && storage_roots) ? storage_roots + 32 * (uint64_t)item : nullptr;
-            uint32_t len = encode_leaf<Strip<BLOCK>, ACCOUNT>(s, k, 0, vp, sp, f.err);
-            meta = strip_to_ref(s, len, false, ref, hashed);
-        } else {
-            uint32_t v = item - (uint32_t)f.n;
-            uint32_t d = f.node_masks[v].w;
-            uint32_t j0 = f.node_start[v], k = f.node_start[v + 1] - j0;
-            uint32_t sm, tm, hm, l, r;
-            uint32_t len = encode_branch_u<BLOCK, 16>(s, f, j0, k, sm, tm, hm, l, r);
-            meta = strip_to_ref(s, len, false, ref, hashed);
-            meta = thread_finish_node(s, ref, meta, 0, (int)d, f.keys + 32 * (uint64_t)l, hashed, exts);
-        }
-        LinBuf lb{e.as_child, 0};
-        put_child(lb, ref, meta & META_LEN);
-        e.as_child_len = (uint8_t)lb.n;
-    }
+    if (lo < hi) frontier_entry<BLOCK, ACCOUNT, false>(s, f, f.S[lo], values, storage_roots, nullptr, e);
 }
 
 // Root from the gathered 16-entry frontier (single thread).

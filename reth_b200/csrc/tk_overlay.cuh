@@ -160,13 +160,15 @@ __device__ __forceinline__ uint32_t ov_root_tree(const DTrieDev &t, uint32_t w) 
 // current root).  Threads [n_blocks, n_blocks + m): the storage root of every entry that is live, not wiped, has slots (or,
 // with reveal_targets, is an account target) and whose account exists with a non-empty storage trie — so the storage tries
 // are revealed at the same levels as the account tries.  found (nullable): found[a] = entry a's account is in the account
-// arena.
+// arena.  With bucket_tries the account arena is a shard's 16 bucket tries and every block lies in one bucket: a block
+// starts from its bucket's trie, and an entry's account is looked up in the trie of its top key nibble.
 __global__ void ov_seed_kernel(DTrieDev ta, DTrieDev ts, StatelessDev s, const uint8_t *root, uint8_t *parent, OvNode *q,
                                uint32_t *n_q, SlItem *items, uint32_t *n_items, uint8_t *vals, uint8_t *found) {
     const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < s.n_blocks) {
         for (int k = 0; k < 32; k++) parent[32 * i + k] = root[k];
-        const uint32_t lo = (uint32_t)s.block_acct[i], hi = (uint32_t)s.block_acct[i + 1], w = ta.troot[0];
+        const uint32_t lo = (uint32_t)s.block_acct[i], hi = (uint32_t)s.block_acct[i + 1];
+        const uint32_t w = !s.bucket_tries ? ta.troot[0] : lo < hi ? ta.troot[s.akeys[32 * (uint64_t)lo] >> 4] : DT_NONE;
         if (lo < hi && w != DT_NONE)
             ov_word(ta, s, w, -1, ov_root_tree(ta, w), (uint32_t)(s.m + i), (uint32_t)i, lo, hi, 0, (uint32_t)s.n_t, q, n_q, items, n_items,
                     vals);
@@ -178,7 +180,7 @@ __global__ void ov_seed_kernel(DTrieDev ta, DTrieDev ts, StatelessDev s, const u
     const bool has_slots = s.seg[a + 1] != s.seg[a];
     const bool reveal = (fl & 1) && !(fl & 4) && (has_slots || s.reveal_targets);
     if (!reveal && !found) return;
-    const DtLoc loc = dt_descend(ta, 0, s.akeys + 32 * a);
+    const DtLoc loc = dt_descend(ta, s.bucket_tries ? (uint32_t)(s.akeys[32 * a] >> 4) : 0u, s.akeys + 32 * a);
     if (found) found[a] = loc.found ? 1 : 0;
     if (!reveal || !loc.found) return;
     const uint32_t w = ts.troot[loc.child & ~DT_LEAF];
@@ -255,6 +257,44 @@ __global__ void ov_removed_paths_kernel(DTrieDev t, const uint32_t *__restrict__
     for (uint32_t b = 0; b < 32; b++) pp[b] = (uint8_t)(2 * b + 1 < d ? key[b] : (2 * b < d ? (key[b] & 0xF0) : 0));
     path_len[i] = (uint8_t)d;
     trie_id[i] = cand[2 * i] - trie_base;
+}
+
+// b200_dstate_overlay_frontiers: thread 16 b + k writes the entry of bucket k after block b.  seg[v] (the fold's account
+// segments) of virtual block v = vblock[16 b + k], block b's entries in bucket k, is the bucket's trie after the block;
+// vblock < 0: the block does not touch the bucket, which keeps its entry of `cur`.  An empty segment is a bucket the block
+// empties: an all-zero entry.
+template <int BLOCK>
+__global__ void __launch_bounds__(BLOCK) ov_frontier_kernel(ForestDev f, const uint64_t *__restrict__ seg, const int32_t *__restrict__ vblock,
+                                                           uint64_t n, const uint8_t *__restrict__ values, const uint8_t *__restrict__ sroots,
+                                                           const uint8_t *__restrict__ nibs, const FrontierEntryDev *__restrict__ cur,
+                                                           FrontierEntryDev *__restrict__ out) {
+    extern __shared__ uint32_t smem[];
+    const uint64_t i = (uint64_t)blockIdx.x * BLOCK + threadIdx.x;
+    Strip<BLOCK> s;
+    s.init(smem);
+    if (i >= n || *(volatile int *)f.err != B200_DEVERR_NONE) return;
+    const int32_t v = vblock[i];
+    FrontierEntryDev &e = out[i];
+    if (v < 0) {
+        e = cur[i & 15];
+        return;
+    }
+    for (int k = 0; k < 33; k++) e.as_child[k] = e.as_root[k] = 0;
+    e.as_child_len = e.as_root_len = 0;
+    const uint64_t lo = seg[v], hi = seg[v + 1];
+    if (lo < hi) frontier_entry<BLOCK, true, true>(s, f, f.S[lo], values, sroots, nibs, e);
+}
+
+cudaError_t launch_ov_frontier(const ForestDev &f, const uint64_t *seg, const int32_t *vblock, uint64_t n, const uint8_t *values,
+                               const uint8_t *sroots, const uint8_t *nibs, const FrontierEntryDev *cur, FrontierEntryDev *out,
+                               cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    constexpr int B = 32;
+    auto k = ov_frontier_kernel<B>;
+    const size_t smem = (size_t)BRANCH_WORDS * B * 4;
+    cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    k<<<blocks_for(n, B), B, smem, st>>>(f, seg, vblock, n, values, sroots, nibs, cur, out);
+    return cudaGetLastError();
 }
 
 cudaError_t launch_ov_seed(const DTrieDev &ta, const DTrieDev &ts, const StatelessDev &s, const uint8_t *root, uint8_t *parent, OvNode *q,

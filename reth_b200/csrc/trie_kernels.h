@@ -366,6 +366,7 @@ struct StatelessDev {
     const uint8_t *tskeys;       // [tseg[n_t]][32]
     uint64_t n_t;
     int reveal_targets;          // overlay witness: an entry whose key is an account target also reveals its storage without slots
+    int bucket_tries;            // overlay frontiers: the account arena holds 16 top-nibble bucket tries, each block lies in one
 };
 struct SlNode {  // a queued node: trie, path (packed nibbles, zero-padded) and depth, RLP at rlp[off, off + len)
     uint8_t path[32];
@@ -420,6 +421,11 @@ cudaError_t launch_ov_reveal(const DTrieDev &ta, const DTrieDev &ts, const State
                              uint32_t *n_next, SlItem *items, uint32_t *n_items, uint8_t *vals, OvRemoved rm, cudaStream_t st);
 cudaError_t launch_ov_removed_paths(const DTrieDev &t, const uint32_t *cand, uint32_t n, uint32_t trie_base, uint8_t *path_len,
                                     uint8_t *path_packed, uint32_t *trie_id, cudaStream_t st);
+// b200_dstate_overlay_frontiers: the n = 16 x blocks entries from the account fold f (segments seg, rows values / sroots /
+// nibs) and the current frontier cur; vblock[i]: the segment of entry i, or -1 (cur[i % 16])
+cudaError_t launch_ov_frontier(const ForestDev &f, const uint64_t *seg, const int32_t *vblock, uint64_t n, const uint8_t *values,
+                               const uint8_t *sroots, const uint8_t *nibs, const FrontierEntryDev *cur, FrontierEntryDev *out,
+                               cudaStream_t st);
 
 cudaError_t launch_dt_restructure_fused(const DTrieDev &t, const uint32_t *trie_of_key, const uint8_t *keys, const uint8_t *vals,
                                         const uint8_t *flags, const uint8_t *sroots, uint32_t m, uint8_t *kind, uint32_t *leaf_of,

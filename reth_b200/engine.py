@@ -1078,6 +1078,17 @@ class DynamicState:
                         deleted[lo:hi].copy()))
         return out
 
+    def overlay_frontiers(self, blocks) -> np.ndarray:
+        """b200_dstate_overlay_frontiers, on a sharded state: (n, 16, 68) uint8, row b = the entries `frontier()` would return
+        after `apply` of block b alone; the state does not change.  blocks: as for `overlay_roots` (this shard's part of
+        each block).  The ranks gather the rows and Engine.root_from_frontier of block b's merged entries is its root."""
+        args = block_batch_arrays(blocks)
+        n = len(blocks)
+        out = (FrontierEntry * (16 * max(n, 1)))()
+        self.engine._check(self.engine.lib.b200_dstate_overlay_frontiers(self.handle, n, *(_ptr(a) for a in args), out,
+                                                                         C.byref(Stats())))
+        return np.frombuffer(bytes(out), np.uint8).reshape(-1, 16, 68)[:n].copy()
+
     def trie_changesets(self, acct_paths, storage: dict) -> tuple:
         """b200_dstate_trie_changesets: the values the changed trie nodes of a block had before it, against the state as it
         is (the state does not change; reth's compute_trie_changesets).  acct_paths: the block's changed account-trie paths

@@ -8,13 +8,13 @@ between ranks: this is the collective-free partitioning of the reference's Paral
 (crates/trie/parallel/src/root.rs:101-127) carried over to the live path."""
 from __future__ import annotations
 
-from typing import Tuple
+from typing import List, Tuple
 
 import numpy as np
 
 from .engine import Engine
 from .hashed_state import HashedPostState, HashedPostStateSorted
-from .trie import DynamicStateRoot, TrieUpdates
+from .trie import DynamicStateRoot, StateRootError, TrieUpdates, apply_layout
 
 
 def owner_of(key: bytes, world: int) -> int:
@@ -37,29 +37,64 @@ class ShardedDynamicStateRoot:
     def root(self) -> bytes:
         return self._root
 
-    def _gather_root(self) -> bytes:
-        if self.comm is not None:
-            return self.comm.dstate_root_sharded(self.local.ds)
+    def _all_gather(self, fr: np.ndarray) -> np.ndarray:
+        """fr: this rank's frontier rows (..., 16, 68) uint8 -> (world, ..., 16, 68), every rank's (torch.distributed)."""
+        if self.world == 1:
+            return fr[None]
         import torch
         import torch.distributed as dist
-        fr = self.local.ds.frontier()                                  # (16, 68) uint8, empty outside this rank's buckets
-        if self.world == 1:
-            return self.engine.root_from_frontier(fr)
         dev = "cuda" if dist.get_backend(self.group) == "nccl" else "cpu"
-        mine = torch.from_numpy(fr.reshape(-1)).to(dev)
+        mine = torch.from_numpy(np.ascontiguousarray(fr).reshape(-1)).to(dev)
         gathered = [torch.empty_like(mine) for _ in range(self.world)]
         dist.all_gather(gathered, mine, group=self.group)
-        allf = torch.stack(gathered).view(self.world, 16, 68).cpu().numpy()
+        return torch.stack(gathered).cpu().numpy().reshape((self.world,) + fr.shape)
+
+    def _merged_root(self, allf: np.ndarray) -> bytes:
+        """allf: (world, 16, 68), every rank's entries -> the state root from the owner's entry of every bucket."""
         pick = np.arange(16) * self.world // 16                       # owner of every bucket (same map as bench.py)
         return self.engine.root_from_frontier(np.ascontiguousarray(allf[pick, np.arange(16)]))
 
+    def _gather_root(self) -> bytes:
+        if self.comm is not None:
+            return self.comm.dstate_root_sharded(self.local.ds)
+        fr = self.local.ds.frontier()                                  # (16, 68) uint8, empty outside this rank's buckets
+        if self.world == 1:
+            return self.engine.root_from_frontier(fr)
+        return self._merged_root(self._all_gather(fr))
+
+    def _part(self, post: HashedPostState) -> HashedPostState:
+        return HashedPostState({k: a for k, a in post.accounts.items() if owner_of(k, self.world) == self.rank},
+                               {k: s for k, s in post.storages.items() if owner_of(k, self.world) == self.rank})
+
     def commit(self, post: HashedPostState) -> Tuple[bytes, TrieUpdates]:
         """-> (state root, this rank's part of the block's TrieUpdates)."""
-        part = HashedPostState({k: a for k, a in post.accounts.items() if owner_of(k, self.world) == self.rank},
-                               {k: s for k, s in post.storages.items() if owner_of(k, self.world) == self.rank})
-        _, updates = self.local.commit(part)
+        _, updates = self.local.commit(self._part(post))
         self._root = self._gather_root()
         return self._root, updates
+
+    def overlay_roots(self, posts) -> List[bytes]:
+        """The state root `commit` of each post alone would return, with every shard left as it is: payload validation and
+        payload building over a sharded state, before `commit` keeps one block (DynamicStateRoot.overlay_roots on one
+        GPU).  The posts are siblings on the current state, not a chain.  Collective: every rank calls it with the same
+        posts.  Each rank computes its frontier entries after every post (b200_dstate_overlay_frontiers), one all-gather of
+        n x 16 x 68 bytes over torch.distributed exchanges them, and every rank finishes each root with
+        b200_root_from_frontier.  At world > 1 a torch.distributed process group must be initialised, also when the
+        object was made with `comm`: this exchange does not run through the library's NCCL communicator."""
+        if not posts:
+            return []
+        blocks = [apply_layout(self._part(post), destroyed_slots=False)[1] for post in posts]
+        try:
+            fr = self.local.ds.overlay_frontiers(blocks)               # (n, 16, 68)
+        except ValueError:
+            raise
+        except Exception as e:  # noqa: BLE001
+            raise StateRootError(str(e)) from e
+        allf = self._all_gather(fr)                                    # (world, n, 16, 68)
+        return [self._merged_root(allf[:, b]) for b in range(len(posts))]
+
+    def overlay_root(self, post: HashedPostState) -> bytes:
+        """overlay_roots for one post: the state root `commit(post)` would return, without changing any shard."""
+        return self.overlay_roots([post])[0]
 
     def close(self):
         self.local.close()

@@ -35,7 +35,18 @@ block.  Each with its time, launches, read-backs and proof node count (account +
 is a second block of the same shape on top of it.  Alternating rep by rep: the overlay witness; b200_dstate_overlay_roots of
 the overlay block; b200_dstate_witness of the target block on the resident state.  Each with its time, launches, read-backs
 and node count.  Afterwards the overlay block is applied, and b200_dstate_witness of the target on the changed state must
-give the same map and the overlay root."""
+give the same map and the overlay root.
+
+    python tools/overlay_bench.py --shards 4
+
+--shards S measures the overlay frontiers of a sharded state (b200_dstate_overlay_frontiers): the same state as S shards in
+one process on one GPU (rank r owns top nibbles [16r/S, 16(r+1)/S), as reth_b200.sharded does), the first block split by
+owner.  Alternating rep by rep: the overlay-frontiers call of every shard on its part of the block, each timed on its own;
+the root from the merged frontier (b200_root_from_frontier); b200_dstate_overlay_roots of the whole block on the unsharded
+state; and b200_dstate_apply on sharded twins, each shard timed on its own (the first rep applies the first block, every
+later rep a fresh block of the same shape on top).  Reported per shard call: time, and their maximum (what S GPUs would
+spend before the all-gather) and sum; launches and read-backs.  Checked in the run: the merged root equals the unsharded
+overlay root and the twins' root after the block, and every shard keeps its root and frontier."""
 import argparse
 import ctypes as C
 import json
@@ -64,11 +75,13 @@ def main():
     ap.add_argument("--updates", action="store_true", help="measure the overlay with TrieUpdates (see above)")
     ap.add_argument("--proofs", action="store_true", help="measure the overlay multiproof (see above)")
     ap.add_argument("--witness", action="store_true", help="measure the overlay witness (see above)")
+    ap.add_argument("--shards", type=int, nargs="?", const=4, default=0,
+                    help="measure the overlay frontiers of a state in this many shards (default 4; see above)")
     args = ap.parse_args()
     import torch
 
     from reth_b200 import DynamicState, Engine
-    from reth_b200._lib import Proofs, Stats, Updates, Witness
+    from reth_b200._lib import FrontierEntry, Proofs, Stats, Updates, Witness
     from reth_b200.engine import _ptr, block_batch_arrays, witness_batch_arrays
     out = {"card": card()}
     eng = Engine(0)
@@ -148,6 +161,143 @@ def main():
         for k in calls:
             res[k].update({"device_ms": spread(dev[k]), "host_call_ms": spread(host[k])})
         return res
+
+    if args.shards:
+        S = args.shards
+        if not 1 <= S <= 16:
+            raise SystemExit("--shards: 1 to 16")
+        owner = lambda k: (k[:, 0].astype(np.int64) >> 4) * S // 16
+        bounds = np.searchsorted(owner(keys), np.arange(S + 1))       # keys are sorted: every rank holds a run of them
+
+        def state_part(r):
+            lo, hi = int(bounds[r]), int(bounds[r + 1])
+            so = offs[lo:hi + 1]
+            return keys[lo:hi], accs[lo:hi], skeys[int(so[0]):int(so[-1])], svals[int(so[0]):int(so[-1])], so - so[0]
+
+        def block_part(a, r):
+            bb = np.searchsorted(owner(a[0]), np.arange(S + 1))
+            lo, hi = int(bb[r]), int(bb[r + 1])
+            so = np.asarray(a[5], np.uint64)[lo:hi + 1]
+            return (a[0][lo:hi], a[1][lo:hi], a[2][lo:hi], a[3][int(so[0]):int(so[-1])], a[4][int(so[0]):int(so[-1])], so - so[0])
+        shards = [DynamicState.create(eng, *state_part(r), sharded=True) for r in range(S)]
+        twins = [DynamicState.create(eng, *state_part(r), sharded=True) for r in range(S)]
+        pick = np.arange(16) * S // 16                                # owner of every bucket
+
+        def merge(frs):
+            return np.ascontiguousarray(np.stack(frs)[pick, np.arange(16)])
+        shard_root0 = [(d.root(), d.frontier()) for d in shards]
+        assert eng.root_from_frontier(merge([f for _, f in shard_root0])) == parent
+        a0 = arrays[0]
+        packed = [block_batch_arrays([block_part(a0, r)]) for r in range(S)]
+        frs = [(FrontierEntry * 16)() for _ in range(S)]
+        as_np = lambda fr: np.frombuffer(bytes(fr), np.uint8).reshape(16, 68)
+        packed_u, roots = block_batch_arrays([a0]), np.zeros((1, 32), np.uint8)
+
+        def frontiers(r):
+            return lambda: eng._check(eng.lib.b200_dstate_overlay_frontiers(shards[r].handle, 1, *(_ptr(x) for x in packed[r]), frs[r],
+                                                                            C.byref(Stats())))
+
+        def merged_root():
+            return eng.root_from_frontier(merge([as_np(f) for f in frs]))
+
+        def overlay_root():
+            eng._check(eng.lib.b200_dstate_overlay_roots(ds.handle, 1, *(_ptr(x) for x in packed_u), _ptr(roots), C.byref(Stats())))
+        chain = iter([a0] + [block_arrays(make_block(rng, keys, skeys, offs, args.touch, args.slot_writes))
+                             for _ in range(args.warmup + args.reps + 1)])
+        root = np.zeros(32, np.uint8)
+
+        def twin_apply(r):
+            def call():
+                a = cur[r]
+                eng._check(eng.lib.b200_dstate_apply(twins[r].handle, _ptr(a[0]), _ptr(a[1]), _ptr(a[2]), len(a[0]), _ptr(a[3]),
+                                                     _ptr(a[4]), _ptr(a[5]), _ptr(root), None, None, None, None, None, C.byref(Stats())))
+            return call
+        # ---- the cross-checks: merged overlay root == unsharded overlay root == the twins' root after the block
+        for r in range(S):
+            frontiers(r)()
+        overlay_root()
+        a = next(chain)
+        cur = [block_part(a, r) for r in range(S)]
+        for r in range(S):
+            twin_apply(r)()
+        twin_root = eng.root_from_frontier(merge([t.frontier() for t in twins]))
+        assert merged_root() == roots[0].tobytes() == twin_root, "merged overlay root differs"
+        assert [as_np(f).tobytes() for f in frs] == [t.frontier().tobytes() for t in twins], "overlay frontier differs from the apply"
+        # ---- counts of one call each
+        res = {"overlay_frontiers": [counts(frontiers(r)) for r in range(S)], "root_from_frontier": counts(merged_root),
+               "overlay_roots_unsharded": counts(overlay_root)}
+        # ---- timed, alternating rep by rep (warm-ups included in the same loop)
+        t = {"overlay_frontiers": [[] for _ in range(S)], "root_from_frontier": [], "overlay_roots_unsharded": [],
+             "apply_twins": [[] for _ in range(S)]}
+        host_t = {k: [] for k in ("overlay_frontiers", "root_from_frontier", "overlay_roots_unsharded", "apply_twins")}
+
+        def timed(call):
+            torch.cuda.synchronize()
+            ev0.record(stream)
+            t0 = time.perf_counter()
+            call()
+            h = (time.perf_counter() - t0) * 1e3
+            ev1.record(stream)
+            ev1.synchronize()
+            return ev0.elapsed_time(ev1), h
+        apply_launches = []
+        for rep in range(args.warmup + args.reps):
+            keep = rep >= args.warmup
+            hs = 0.0
+            for r in range(S):
+                d, h = timed(frontiers(r))
+                hs += h
+                if keep:
+                    t["overlay_frontiers"][r].append(d)
+            if keep:
+                host_t["overlay_frontiers"].append(hs)
+            for k, call in (("root_from_frontier", merged_root), ("overlay_roots_unsharded", overlay_root)):
+                d, h = timed(call)
+                if keep:
+                    t[k].append(d)
+                    host_t[k].append(h)
+            a = next(chain)
+            cur = [block_part(a, r) for r in range(S)]
+            hs, l0 = 0.0, eng.launch_count()
+            for r in range(S):
+                d, h = timed(twin_apply(r))
+                hs += h
+                if keep:
+                    t["apply_twins"][r].append(d)
+            apply_launches.append(eng.launch_count() - l0)
+            if keep:
+                host_t["apply_twins"].append(hs)
+        for d, (r0, f0) in zip(shards, shard_root0):
+            assert d.root() == r0 and np.array_equal(d.frontier(), f0), "a shard changed"
+        assert merged_root() == roots[0].tobytes()
+
+        def per_shard(xs):
+            xs = np.array(xs)                                          # [shard][rep]
+            return {"per_shard_ms": [spread(x) for x in xs], "max_over_shards_ms": spread(xs.max(axis=0)),
+                    "sum_over_shards_ms": spread(xs.sum(axis=0))}
+        res["overlay_frontiers"] = dict(per_shard(t["overlay_frontiers"]), host_call_ms_all_shards=spread(host_t["overlay_frontiers"]),
+                                        launches=[c["launches"] for c in res["overlay_frontiers"]],
+                                        readbacks_dtoh=[c["readbacks_dtoh"] for c in res["overlay_frontiers"]],
+                                        copies_htod=[c["copies_htod"] for c in res["overlay_frontiers"]])
+        for k in ("root_from_frontier", "overlay_roots_unsharded"):
+            res[k].update({"device_ms": spread(t[k]), "host_call_ms": spread(host_t[k])})
+        res["apply_twins"] = dict(per_shard(t["apply_twins"]), host_call_ms_all_shards=spread(host_t["apply_twins"]),
+                                  launches_all_shards=int(np.median(apply_launches)),
+                                  note="every rep applies a fresh block of the same shape on top of the previous one")
+        out.update(res)
+        out["shards"] = S
+        out["block_accounts_per_shard"] = [int(len(p[0])) for p in packed]
+        mo = out["overlay_roots_unsharded"]["device_ms"]["median"]
+        out["ratios"] = {"max_shard_over_unsharded_overlay": round(out["overlay_frontiers"]["max_over_shards_ms"]["median"] / mo, 2),
+                         "sum_shards_over_unsharded_overlay": round(out["overlay_frontiers"]["sum_over_shards_ms"]["median"] / mo, 2),
+                         "max_shard_overlay_over_max_shard_apply": round(out["overlay_frontiers"]["max_over_shards_ms"]["median"] /
+                                                                         out["apply_twins"]["max_over_shards_ms"]["median"], 2)}
+        out["card_after"] = card()
+        print(json.dumps(out))
+        for d in shards + twins + [ds]:
+            d.close()
+        eng.close()
+        return
 
     if args.proofs:
         a0 = arrays[0]
