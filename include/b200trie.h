@@ -544,7 +544,8 @@ B200_API int32_t b200_dstate_overlay_frontiers(b200_dstate *, uint64_t n_blocks,
  * rlp[rlp_offset[k] .. rlp_offset[k+1]), root first — every node whose position is a prefix of the target key (what
  * alloy-trie's ProofRetainer keeps): extension and branch are separate nodes, the walk ends at a leaf (inclusion, or
  * exclusion by another key), at an empty branch slot or inside a diverging extension.  An empty trie gives the single
- * node 0x80.  Pinned by reth's own vectors (crates/trie/db/tests/proof.rs:44-165).  Not for sharded states. */
+ * node 0x80.  Pinned by reth's own vectors (crates/trie/db/tests/proof.rs:44-165).  Not for sharded states: see
+ * b200_dstate_sharded_multiproof. */
 typedef struct {
     uint64_t n_targets;
     uint64_t *node_offset; /* [n_targets+1] */
@@ -573,6 +574,50 @@ B200_API int32_t b200_dstate_multiproof(b200_dstate *, const uint8_t *acct_keys3
                                         const uint64_t *slot_seg_offsets, const uint8_t *slot_keys32, b200_proofs *account_proofs,
                                         uint8_t *storage_roots32, b200_proofs *storage_proofs);
 B200_API void b200_proofs_release(b200_proofs *);
+/* Proofs over a sharded state (b200_dstate_create_sharded): eth_getProof and the proof workers' Proof::multiproof when the
+ * state is spread over several GPUs.  The depth-0 root branch of the whole state is in no shard; each rank gives its part of
+ * that node (b200_dstate_frontier and b200_dstate_frontier_masks), the ranks all-gather them, and each rank proves the
+ * targets of its own buckets with b200_dstate_sharded_multiproof.
+ *
+ * The bits this shard's buckets set in the masks of the depth-0 root branch of the whole state.
+ * hash bit k: bucket k's top node is a branch at depth 1.
+ * tree bit k: bucket k's top node is a branch that reth stores (tree_mask | hash_mask != 0), at any depth.
+ * Buckets the shard does not hold, leaf tops and empty buckets give 0.  The ranks OR their masks.
+ * An unsharded state gives B200_ERR_INVALID_ARG. */
+B200_API int32_t b200_dstate_frontier_masks(b200_dstate *, uint16_t *hash_mask, uint16_t *tree_mask);
+/* b200_dstate_multiproof on one rank's shard.  merged[16]: the entry of every bucket from its owner, as passed to
+ * b200_root_from_frontier.  root_hash_mask / root_tree_mask: the OR of every rank's b200_dstate_frontier_masks.
+ *
+ * Equality: every output is byte for byte what b200_dstate_multiproof gives for the same targets on an unsharded state of
+ * all accounts: node RLPs, node order, node_depth, node_masks, storage_roots32, and the 0x80 proofs of an absent account's
+ * slots.
+ *
+ * The root, decided by the number of non-empty buckets in merged:
+ *   none: every account proof is the single node 0x80;
+ *   exactly one, bucket j: its trie is the whole trie and every proof walks it from parent depth -1 (its top node is the
+ *     root: an extension over nibble j when the top is a branch), also for targets whose own bucket is empty;
+ *   two or more: node 0 is the root branch, at depth 0, with node_masks hash << 16 | tree (0 when both are 0).  A target
+ *     whose bucket is non-empty continues from that bucket's top node at parent depth 0; for a target whose bucket is
+ *     empty the proof ends with the root branch.
+ *
+ * The answering bucket of a target is its own top nibble when that bucket is non-empty, otherwise in the one-bucket case
+ * that one bucket, otherwise none (any shard can answer).  A shard answers a target only when it holds the answering bucket
+ * or there is none; a target of another shard, storage targets of its account included, is B200_ERR_INVALID_ARG.  The
+ * call never returns a partial proof.
+ *
+ * Checks against the shard's own data, all B200_ERR_INVALID_ARG, so that a stale or foreign frontier cannot give a wrong
+ * proof: for every bucket the shard holds, merged[k] equals its current frontier entry byte for byte (so it is not empty)
+ * and the two mask bits of bit k equal its own; every entry is well formed (as_root_len 0 or 32, as_child_len at most 33,
+ * both zero together) and no mask bit is set for an empty entry.
+ *
+ * Everything else is as for b200_dstate_multiproof: null pointers, offsets and the 2^24 target limit; B200_ERR_INVALID_ARG
+ * for an unsharded state.  On error both b200_proofs are released and zeroed.  The state does not change. */
+B200_API int32_t b200_dstate_sharded_multiproof(b200_dstate *, const b200_frontier_entry merged[16],
+                                                uint16_t root_hash_mask, uint16_t root_tree_mask,
+                                                const uint8_t *acct_keys32, uint64_t n_accounts,
+                                                const uint64_t *slot_seg_offsets, const uint8_t *slot_keys32,
+                                                b200_proofs *account_proofs, uint8_t *storage_roots32,
+                                                b200_proofs *storage_proofs);
 /* Execution witness of one block (reth's TrieWitness::compute, crates/trie/trie/src/witness.rs; what debug_executionWitness
  * and stateless re-execution consume): { keccak(node) -> node RLP } of every trie node needed to apply the block to this
  * state, computed on the device from the resident state, which stays unchanged.  The block comes in exactly the layout of

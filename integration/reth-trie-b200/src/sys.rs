@@ -204,6 +204,13 @@ unsafe extern "C" {
                                   slot_keys32: *const u8, account_proofs: *mut b200_proofs, storage_roots32: *mut u8,
                                   storage_proofs: *mut b200_proofs) -> i32;
     pub fn b200_proofs_release(p: *mut b200_proofs);
+    /// the bits this shard's buckets set in the hash / tree masks of the depth-0 root branch; the ranks OR them
+    pub fn b200_dstate_frontier_masks(state: *mut b200_dstate, hash_mask: *mut u16, tree_mask: *mut u16) -> i32;
+    /// b200_dstate_multiproof on one shard, from the gathered frontier (merged16) and the ORed root masks
+    pub fn b200_dstate_sharded_multiproof(state: *mut b200_dstate, merged16: *const b200_frontier_entry, root_hash_mask: u16,
+                                          root_tree_mask: u16, acct_keys32: *const u8, n_accounts: u64, slot_seg_offsets: *const u64,
+                                          slot_keys32: *const u8, account_proofs: *mut b200_proofs, storage_roots32: *mut u8,
+                                          storage_proofs: *mut b200_proofs) -> i32;
     /// multiproof of the state after one candidate block (layout of b200_dstate_apply), the state unchanged
     pub fn b200_dstate_overlay_multiproof(state: *mut b200_dstate, acct_keys32: *const u8, accts: *const b200_account,
                                           acct_flags: *const u8, m: u64, slot_keys32: *const u8, values32_be: *const u8,

@@ -224,6 +224,9 @@ def load():
     sig("b200_dstate_account_proofs", i32, vp, vp, u64, C.POINTER(Proofs))
     sig("b200_dstate_storage_proofs", i32, vp, vp, vp, u64, vp, C.POINTER(Proofs))
     sig("b200_dstate_multiproof", i32, vp, vp, u64, vp, vp, C.POINTER(Proofs), vp, C.POINTER(Proofs))
+    sig("b200_dstate_frontier_masks", i32, vp, C.POINTER(C.c_uint16), C.POINTER(C.c_uint16))
+    sig("b200_dstate_sharded_multiproof", i32, vp, C.POINTER(FrontierEntry), C.c_uint16, C.c_uint16, vp, u64, vp, vp,
+        C.POINTER(Proofs), vp, C.POINTER(Proofs))
     sig("b200_proofs_release", None, C.POINTER(Proofs))
     sig("b200_dstate_witness", i32, vp, vp, vp, vp, u64, vp, vp, vp, i32, i32, C.POINTER(Witness))
     sig("b200_witness_release", None, C.POINTER(Witness))

@@ -40,6 +40,27 @@ __global__ void __launch_bounds__(512) dt_frontier_kernel(DTrieDev t, const uint
     }
 }
 
+// The bits this shard's buckets set in the masks of the depth-0 root branch: out[0] the hash mask, out[1] the tree mask
+// (16 threads, thread k = bucket k).  The rule of dt_branch_payload at depth 0: the top node is a hashed child when it is a
+// branch at depth 1, and a stored one when either of its own masks is set.  The top node's META_EXT is no help here: its
+// reference was built with parent depth -1, as the root of its own trie.
+__global__ void dt_frontier_masks_kernel(DTrieDev t, uint16_t *__restrict__ out) {
+    const uint32_t k = threadIdx.x;
+    const uint32_t w = t.troot[k];
+    const bool node = w != DT_NONE && !(w & DT_LEAF);
+    const bool hash = node && t.ndepth[w] == 1;
+    bool tree = false;
+    if (node) {
+        const ushort4 mk = t.nmasks[w];
+        tree = (mk.y | mk.z) != 0;
+    }
+    const uint32_t hm = __ballot_sync(0xFFFFu, hash), tm = __ballot_sync(0xFFFFu, tree);
+    if (k == 0) {
+        out[0] = (uint16_t)hm;
+        out[1] = (uint16_t)tm;
+    }
+}
+
 // ------------------------------------------------------------------------------------------------ dynamic state glue
 // Which storage tries a block wipes: the tries of destroyed accounts and of accounts flagged "storage wiped"
 // (HashedStorage::wiped, crates/trie/common/src/hashed_state.rs:423-428).  Trie id = id of the account's leaf.

@@ -149,6 +149,26 @@ cudaError_t launch_dt_proof_write(const DTrieDev &t, const DTrieDev &alt, const 
                                                                   node_masks);
     return cudaGetLastError();
 }
+cudaError_t launch_dt_sharded_proof_sizes(const DTrieDev &t, const ShardRootDev &r, const uint8_t *keys, uint64_t n, uint32_t *node_count,
+                                          uint64_t *byte_count, cudaStream_t st) {
+    if (n) dt_sharded_proof_size_kernel<<<blocks_for(n, 64), 64, 0, st>>>(t, r, keys, n, node_count, byte_count);
+    return cudaGetLastError();
+}
+cudaError_t launch_dt_sharded_proof_write(const DTrieDev &t, const ShardRootDev &r, const uint8_t *keys, uint64_t n, const uint64_t *node_base,
+                                          const uint64_t *byte_base, uint8_t *rlp, uint64_t *rlp_offset, uint8_t *node_depth,
+                                          uint32_t *node_masks, cudaStream_t st) {
+    if (n) dt_sharded_proof_write_kernel<<<blocks_for(n, 64), 64, 0, st>>>(t, r, keys, n, node_base, byte_base, rlp, rlp_offset, node_depth,
+                                                                          node_masks);
+    return cudaGetLastError();
+}
+cudaError_t launch_dt_frontier_masks(const DTrieDev &t, uint16_t *out, cudaStream_t st) {
+    dt_frontier_masks_kernel<<<1, 16, 0, st>>>(t, out);
+    return cudaGetLastError();
+}
+cudaError_t launch_root_branch(const FrontierEntryDev *fr, uint8_t *out, cudaStream_t st) {
+    root_branch_kernel<<<1, 1, 0, st>>>(fr, out);
+    return cudaGetLastError();
+}
 cudaError_t launch_dt_find_leaves(const DTrieDev &t, const uint8_t *keys, uint64_t n, uint32_t *leaf_out, uint8_t *sroot_out, cudaStream_t st) {
     if (n) dt_find_leaves_kernel<<<blocks_for(n, 128), 128, 0, st>>>(t, keys, n, leaf_out, sroot_out);
     return cudaGetLastError();

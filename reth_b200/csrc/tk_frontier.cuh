@@ -67,6 +67,30 @@ __global__ void frontier_kernel(ForestDev f, const uint64_t *__restrict__ bucket
     if (lo < hi) frontier_entry<BLOCK, ACCOUNT, false>(s, f, f.S[lo], values, storage_roots, nullptr, e);
 }
 
+// The depth-0 root branch over a gathered frontier with two or more non-empty entries: every bucket's as_child (0x80 for an
+// empty one) and an empty value; at most 3 + 16 x 33 + 1 = 532 bytes.
+template <class W>
+__device__ __forceinline__ void put_root_branch(W &s, const FrontierEntryDev *__restrict__ fr) {
+    uint32_t payload = 1;
+    for (uint32_t b = 0; b < 16; b++) payload += fr[b].as_child_len ? fr[b].as_child_len : 1;
+    put_list_header(s, payload);
+    for (uint32_t b = 0; b < 16; b++) {
+        if (fr[b].as_child_len == 0) s.byte(0x80);
+        else
+            for (uint32_t i = 0; i < fr[b].as_child_len; i++) s.byte(fr[b].as_child[i]);
+    }
+    s.byte(0x80);
+}
+
+// Proofs of a sharded state (b200_dstate_sharded_multiproof): the root branch of the merged frontier as a proof node,
+// its length (u32) at out and its RLP at out + 4 (single thread).
+__global__ void root_branch_kernel(const FrontierEntryDev *__restrict__ fr, uint8_t *__restrict__ out) {
+    if (threadIdx.x != 0) return;
+    LinBuf lb{out + 4, 0};
+    put_root_branch(lb, fr);
+    *reinterpret_cast<uint32_t *>(out) = lb.n;
+}
+
 // Root from the gathered 16-entry frontier (single thread).
 template <int BLOCK>
 __global__ void root_from_frontier_kernel(const FrontierEntryDev *__restrict__ fr, uint8_t *__restrict__ root) {
@@ -90,15 +114,7 @@ __global__ void root_from_frontier_kernel(const FrontierEntryDev *__restrict__ f
             ref[i] = p[0] | (p[1] << 8) | (p[2] << 16) | ((uint32_t)p[3] << 24);
         }
     } else {
-        uint32_t payload = 1;
-        for (uint32_t b = 0; b < 16; b++) payload += fr[b].as_child_len ? fr[b].as_child_len : 1;
-        put_list_header(s, payload);
-        for (uint32_t b = 0; b < 16; b++) {
-            if (fr[b].as_child_len == 0) s.byte(0x80);
-            else
-                for (uint32_t i = 0; i < fr[b].as_child_len; i++) s.byte(fr[b].as_child[i]);
-        }
-        s.byte(0x80);
+        put_root_branch(s, fr);
         uint32_t blocks = s.finish();
         strip_keccak(s, blocks, ref);
     }

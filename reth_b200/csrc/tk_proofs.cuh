@@ -230,6 +230,52 @@ __global__ void dt_proof_write_kernel(DTrieDev t, DTrieDev alt, const uint32_t *
                             node_masks, node_base[i]);
     }
 }
+
+// ---- proofs of a sharded state: the account arena holds the 16 bucket tries, the depth-0 root branch above them is in no
+// arena (ShardRootDev, trie_kernels.h).  With the root branch, the proof is that node, then the walk from the top of the
+// key's bucket at parent depth 0 (nothing more when the bucket is empty); with `only` the bucket's trie is the whole trie.
+template <bool WRITE>
+static __device__ void dt_sharded_proof_walk(const DTrieDev &t, const ShardRootDev &r, const uint8_t *key, uint32_t &n_nodes,
+                                             uint64_t &n_bytes, uint8_t *rlp, uint64_t byte_base, uint64_t *rlp_offset,
+                                             uint8_t *node_depth, uint32_t *node_masks, uint64_t node_base) {
+    if (r.only >= 0) {
+        dt_proof_walk<WRITE>(t, (uint32_t)r.only, key, n_nodes, n_bytes, rlp, byte_base, rlp_offset, node_depth, node_masks, node_base);
+        return;
+    }
+    const uint32_t len = *reinterpret_cast<const uint32_t *>(r.branch);
+    if (WRITE) {
+        for (uint32_t b = 0; b < len; b++) rlp[byte_base + b] = r.branch[4 + b];
+        rlp_offset[node_base] = byte_base;
+        node_depth[node_base] = 0;
+        node_masks[node_base] = r.masks;
+    }
+    n_nodes = 1;
+    n_bytes = len;
+    const uint32_t cur = t.troot[key[0] >> 4];
+    if (cur != DT_NONE)
+        dt_proof_steps<WRITE>(t, cur, 0, key, n_nodes, n_bytes, rlp, byte_base, rlp_offset, node_depth, node_masks, node_base, 0, 0);
+}
+__global__ void dt_sharded_proof_size_kernel(DTrieDev t, ShardRootDev r, const uint8_t *__restrict__ keys, uint64_t n,
+                                             uint32_t *__restrict__ node_count, uint64_t *__restrict__ byte_count) {
+    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    uint32_t nn;
+    uint64_t nb;
+    dt_sharded_proof_walk<false>(t, r, keys + 32 * i, nn, nb, nullptr, 0, nullptr, nullptr, nullptr, 0);
+    node_count[i] = nn;
+    byte_count[i] = nb;
+}
+__global__ void dt_sharded_proof_write_kernel(DTrieDev t, ShardRootDev r, const uint8_t *__restrict__ keys, uint64_t n,
+                                              const uint64_t *__restrict__ node_base, const uint64_t *__restrict__ byte_base,
+                                              uint8_t *__restrict__ rlp, uint64_t *__restrict__ rlp_offset,
+                                              uint8_t *__restrict__ node_depth, uint32_t *__restrict__ node_masks) {
+    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    uint32_t nn;
+    uint64_t nb;
+    dt_sharded_proof_walk<true>(t, r, keys + 32 * i, nn, nb, rlp, byte_base[i], rlp_offset, node_depth, node_masks, node_base[i]);
+}
+
 // the account leaf (= storage trie id) of one account key, DT_NONE when the account does not exist
 __global__ void dt_find_leaf_kernel(DTrieDev t, const uint8_t *__restrict__ key, uint32_t *__restrict__ out, uint64_t n_copies) {
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;

@@ -271,6 +271,21 @@ cudaError_t launch_dt_proof_sizes(const DTrieDev &t, const DTrieDev &alt, const 
 cudaError_t launch_dt_proof_write(const DTrieDev &t, const DTrieDev &alt, const uint32_t *trie_of_target, const uint8_t *keys, uint64_t n,
                                   const uint64_t *node_base, const uint64_t *byte_base, uint8_t *rlp, uint64_t *rlp_offset,
                                   uint8_t *node_depth, uint32_t *node_masks, cudaStream_t st);
+// Account proofs of a sharded state (b200_dstate_sharded_multiproof): `only` >= 0 when at most one bucket of the whole
+// state is non-empty (its trie, or the empty trie 0x80 when none is, is then the whole trie); -1: every proof starts with
+// the depth-0 root branch, its length (u32) at `branch` and its RLP at branch + 4 (device memory), masks hash << 16 | tree.
+struct ShardRootDev {
+    const uint8_t *branch;
+    uint32_t masks;
+    int32_t only;
+};
+cudaError_t launch_dt_sharded_proof_sizes(const DTrieDev &t, const ShardRootDev &r, const uint8_t *keys, uint64_t n, uint32_t *node_count,
+                                          uint64_t *byte_count, cudaStream_t st);
+cudaError_t launch_dt_sharded_proof_write(const DTrieDev &t, const ShardRootDev &r, const uint8_t *keys, uint64_t n, const uint64_t *node_base,
+                                          const uint64_t *byte_base, uint8_t *rlp, uint64_t *rlp_offset, uint8_t *node_depth,
+                                          uint32_t *node_masks, cudaStream_t st);
+cudaError_t launch_dt_frontier_masks(const DTrieDev &t, uint16_t *out, cudaStream_t st);
+cudaError_t launch_root_branch(const FrontierEntryDev *fr, uint8_t *out, cudaStream_t st);
 cudaError_t launch_dt_find_leaves(const DTrieDev &t, const uint8_t *keys, uint64_t n, uint32_t *leaf_out, uint8_t *sroot_out, cudaStream_t st);
 cudaError_t launch_dt_target_tries(const uint64_t *seg_offsets, uint64_t n_accounts, const uint32_t *leaf_of, uint64_t n_targets,
                                    uint32_t *trie_of_target, cudaStream_t st);

@@ -992,6 +992,27 @@ class DynamicState:
                                                                   C.byref(ps)))
         return self._multiproof_dict(addrs, so, slots, pa, sroots, ps, with_nodes)
 
+    def frontier_masks(self) -> tuple:
+        """b200_dstate_frontier_masks, on a sharded state: (hash_mask, tree_mask), the bits this shard's buckets set in the
+        masks of the depth-0 root branch of the whole state.  The ranks OR them."""
+        h, t = C.c_uint16(), C.c_uint16()
+        self.engine._check(self.engine.lib.b200_dstate_frontier_masks(self.handle, C.byref(h), C.byref(t)))
+        return h.value, t.value
+
+    def sharded_multiproof(self, merged, hash_mask: int, tree_mask: int, targets: dict, with_nodes: bool = False) -> dict:
+        """b200_dstate_sharded_multiproof: multiproof(targets) of the whole state, from this shard.  merged: (16, 68) uint8,
+        the owner's frontier entry of every bucket (as for Engine.root_from_frontier); hash_mask / tree_mask: the OR of every
+        rank's frontier_masks().  Every target must be one this shard answers (include/b200trie.h).  -> the dict of
+        multiproof(), equal to multiproof() of the same targets on an unsharded state of all accounts."""
+        fr = (FrontierEntry * 16).from_buffer_copy(_np(merged).reshape(16, 68).tobytes())
+        addrs, ak, so, sk, slots = self._multiproof_targets(targets)
+        n = len(addrs)
+        sroots = np.zeros((max(n, 1), 32), np.uint8)
+        pa, ps = Proofs(), Proofs()
+        self.engine._check(self.engine.lib.b200_dstate_sharded_multiproof(self.handle, fr, hash_mask, tree_mask, _ptr(ak), n, _ptr(so),
+                                                                          _ptr(sk), C.byref(pa), _ptr(sroots), C.byref(ps)))
+        return self._multiproof_dict(addrs, so, slots, pa, sroots, ps, with_nodes)
+
     def overlay_multiproof(self, block, targets: dict, with_nodes: bool = False) -> dict:
         """b200_dstate_overlay_multiproof: multiproof(targets) of the state after `block`, against the state as it is (the
         state does not change; Proof::overlay_multiproof).  block: an `apply` array tuple (acct_keys, accounts, flags,

@@ -96,6 +96,49 @@ class ShardedDynamicStateRoot:
         """overlay_roots for one post: the state root `commit(post)` would return, without changing any shard."""
         return self.overlay_roots([post])[0]
 
+    def multiproof(self, targets: dict) -> dict:
+        """Proof::multiproof(MultiProofTargets) of the whole state: eth_getProof and the proof workers of the state-root task
+        over a sharded state.  targets: {hashed address: iterable of hashed slots}.  -> on every rank, the dict
+        DynamicState.multiproof gives on one GPU.  Collective: every rank calls it with the same targets.  One all-gather
+        of every rank's 16 x 68 frontier bytes and its 4 root-mask bytes gives the root branch; each target goes to the
+        owner of its top nibble (in the one-bucket case, to that bucket's owner), each rank proves its share
+        (b200_dstate_sharded_multiproof), and one all_gather_object of the partial dicts is merged.  At world > 1 a
+        torch.distributed process group must be initialised, also when the object was made with `comm`."""
+        ds = self.local.ds
+        try:
+            hm, tm = ds.frontier_masks()
+            mine = np.concatenate([ds.frontier().reshape(-1), np.array([hm, tm], "<u2").view(np.uint8)])
+        except Exception as e:  # noqa: BLE001
+            raise StateRootError(str(e)) from e
+        allf = self._all_gather(mine)                                  # (world, 16 x 68 + 4)
+        masks = allf[:, 16 * 68:].copy().view("<u2")                   # (world, 2)
+        hash_mask, tree_mask = (int(np.bitwise_or.reduce(masks[:, i])) for i in range(2))
+        frs = allf[:, :16 * 68].reshape(self.world, 16, 68)
+        merged = np.ascontiguousarray(frs[np.arange(16) * self.world // 16, np.arange(16)])   # owner's entry of every bucket
+        nonempty = [k for k in range(16) if merged[k, 34]]             # as_root_len
+        def owner(key: bytes) -> int:
+            k = key[0] >> 4
+            if k not in nonempty and len(nonempty) == 1:
+                k = nonempty[0]
+            return k * self.world // 16
+        share = {a: s for a, s in targets.items() if owner(bytes(a)) == self.rank}
+        try:
+            part = ds.sharded_multiproof(merged, hash_mask, tree_mask, share)
+        except ValueError:
+            raise
+        except Exception as e:  # noqa: BLE001
+            raise StateRootError(str(e)) from e
+        if self.world == 1:
+            return part
+        import torch.distributed as dist
+        parts = [None] * self.world
+        dist.all_gather_object(parts, part, group=self.group)
+        out = {"account_subtree": {}, "branch_node_masks": {}, "storages": {}}
+        for p in parts:
+            for name in out:
+                out[name].update(p[name])
+        return out
+
     def close(self):
         self.local.close()
 
