@@ -636,7 +636,7 @@ B200_API int32_t b200_dstate_sharded_multiproof(b200_dstate *, const b200_fronti
  * Canonical drops every 0x80 node.  An empty block (m = 0) gives the empty map, or with always_include_root the single
  * entry { state root: root node } ({ EMPTY_ROOT_HASH: 0x80 } for an empty state).  Entries are sorted by hash, without
  * duplicates: entry i is hashes32[32i ..], rlp[rlp_offset[i] .. rlp_offset[i+1]).  Keys must be strictly ascending
- * (B200_ERR_UNSORTED).  Not for sharded states (B200_ERR_INVALID_ARG). */
+ * (B200_ERR_UNSORTED).  Not for sharded states (B200_ERR_INVALID_ARG): see b200_dstate_sharded_witness. */
 enum { B200_WITNESS_LEGACY = 0, B200_WITNESS_CANONICAL = 1 };
 typedef struct {
     uint64_t n;
@@ -649,6 +649,58 @@ B200_API int32_t b200_dstate_witness(b200_dstate *, const uint8_t *acct_keys32, 
                                      uint64_t m, const uint8_t *slot_keys32, const uint8_t *values32_be, const uint64_t *seg_offsets,
                                      int32_t mode, int32_t always_include_root, b200_witness *out);
 B200_API void b200_witness_release(b200_witness *);
+/* The execution witness of a block over a sharded state (b200_dstate_create_sharded): debug_executionWitness, the
+ * invalid-block witness hook and stateless clients when the state is spread over several GPUs.  Each rank passes its part
+ * of the block; the union of the ranks' maps, duplicates removed, is byte for byte the map b200_dstate_witness gives for the
+ * whole block on an unsharded state of all accounts, in both modes, and every rank's map is a subset of it.  The depth-0
+ * root branch is in no shard, and whether it keeps a single child after the removal phase is the one decision no shard
+ * makes alone: each rank gives its kept mask (b200_dstate_witness_root_kept), and the ranks OR the masks and all-gather
+ * them with the frontier (b200_dstate_frontier) and the root masks (b200_dstate_frontier_masks).
+ *
+ * This shard's kept mask for its part of the block (a block in the b200_dstate_apply layout, as b200_dstate_witness takes
+ * it).  The entries are routed by their own top nibble; an entry of a bucket this shard does not hold counts as an absent
+ * account.  Bit k: after the mode's removal phase (Legacy: the removals; Canonical: the upserts, then the removals) bucket
+ * k still holds a leaf: the shard holds bucket k and not every leaf of it is removed, or in Canonical mode the part inserts
+ * a live account into bucket k.  The OR of every rank's mask, each over the entries of its own buckets, is the set of
+ * surviving children of the unsharded root branch.  Errors as b200_dstate_witness (*kept is then 0); an unsharded state is
+ * B200_ERR_INVALID_ARG.  The state does not change. */
+B200_API int32_t b200_dstate_witness_root_kept(b200_dstate *, const uint8_t *acct_keys32, const b200_account *accts,
+                                               const uint8_t *acct_flags, uint64_t m, const uint8_t *slot_keys32,
+                                               const uint8_t *values32_be, const uint64_t *seg_offsets, int32_t mode, uint16_t *kept);
+/* b200_dstate_witness on one rank's shard.  merged, root_hash_mask, root_tree_mask: as for b200_dstate_sharded_multiproof;
+ * root_kept: the OR of every rank's b200_dstate_witness_root_kept (for the same block and mode).
+ *
+ * The rule of b200_dstate_witness, split by the number of non-empty buckets in merged:
+ *   none: the state is empty, every proof is the single node 0x80 (dropped in Canonical mode);
+ *   exactly one, bucket j: its trie is the whole trie, walked from parent depth -1 (the root is an extension over nibble j
+ *     when its top is a branch; both nodes belong to the witness), removal reveals included, also at the top branch;
+ *   two or more: every account proof starts with the depth-0 root branch and goes on from the top of the key's own bucket
+ *     at parent depth 0 (nothing more when that bucket is empty).  The reveal at depth 0 applies when root_kept has the
+ *     single bit c, merged[c] is hashed (as_child_len 33) and no entry of the block has top nibble c: the owner of bucket c
+ *     then adds the proof of c ‖ 0…0 from depth 1 on.
+ * Storage targets, the Legacy storage-root nodes and the wipe expansion stay in the shard that owns the account.
+ *
+ * An entry belongs to the owner of its own bucket when that bucket is non-empty in merged, in the one-bucket case to the
+ * owner of that bucket, and with no bucket to any shard; an entry of another shard, its slots included, is
+ * B200_ERR_INVALID_ARG.  With two or more buckets, an entry whose bucket is empty in merged belongs to every shard: every
+ * part holds it (its nodes are the same from any shard, and the union removes the duplicates).  A part without entries gives the empty map, or with always_include_root the single entry { state
+ * root: root node } (in the one-bucket case only from the owner of that bucket; the others give the empty map), unless the
+ * shard owes the depth-0 reveal.  The caller sets always_include_root only when the whole block is empty: on an empty state
+ * in Canonical mode a part's root entry would otherwise be a 0x80 the unsharded map drops.
+ *
+ * Checks, all B200_ERR_INVALID_ARG: those of b200_dstate_sharded_multiproof on merged and the masks, and these on root_kept:
+ *   - for every bucket k this shard holds, bit k equals the kept bit this call computes for its part;
+ *   - for every bucket k empty in merged: in Legacy mode bit k is 0; in Canonical mode with two or more buckets, bit k is
+ *     set exactly when this part inserts a live account into bucket k.
+ * So every bit of root_kept is checked by some rank (a non-empty bucket's by its owner, an empty bucket's by every rank):
+ * a stale or foreign kept mask makes at least one rank's call fail, and never makes all of them succeed with a wrong
+ * union.  (With fewer than two buckets the mask does not enter the witness.)  Everything else is as for b200_dstate_witness (B200_ERR_UNSORTED, the 2^24 limit, the modes).  On
+ * any error out is released and zeroed.  The state does not change.  opt_stats (nullable): the call's counters. */
+B200_API int32_t b200_dstate_sharded_witness(b200_dstate *, const b200_frontier_entry merged[16], uint16_t root_hash_mask,
+                                             uint16_t root_tree_mask, uint16_t root_kept, const uint8_t *acct_keys32,
+                                             const b200_account *accts, const uint8_t *acct_flags, uint64_t m,
+                                             const uint8_t *slot_keys32, const uint8_t *values32_be, const uint64_t *seg_offsets,
+                                             int32_t mode, int32_t always_include_root, b200_witness *out, b200_stats *opt_stats);
 /* Post-block state roots from execution witnesses: stateless validation (reth: DecodedMultiProofV2::from_witness,
  * crates/trie/common/src/proofs.rs:469-544, revealed into a SparseStateTrie and updated, crates/trie/sparse/src/state.rs).
  * A batch of n_blocks independent blocks, each with its own parent state root and witness; no b200_dstate is involved.

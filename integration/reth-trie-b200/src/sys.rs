@@ -233,6 +233,18 @@ unsafe extern "C" {
                                        storage_path_packed: *const u8, account_out: *mut b200_updates,
                                        storage_out: *mut b200_updates, opt_stats: *mut b200_stats) -> i32;
     pub fn b200_witness_release(w: *mut b200_witness);
+    /// this shard's kept mask for its part of a block (the entries of its own buckets): bit k = bucket k still holds a
+    /// leaf after the mode's removal phase; the ranks OR the masks for b200_dstate_sharded_witness
+    pub fn b200_dstate_witness_root_kept(state: *mut b200_dstate, acct_keys32: *const u8, accts: *const b200_account,
+                                         acct_flags: *const u8, m: u64, slot_keys32: *const u8, values32_be: *const u8,
+                                         seg_offsets: *const u64, mode: i32, kept: *mut u16) -> i32;
+    /// b200_dstate_witness of one shard's part of a block, from the gathered frontier (merged16), the ORed root masks and
+    /// the ORed kept masks; the union of the ranks' maps is the unsharded witness
+    pub fn b200_dstate_sharded_witness(state: *mut b200_dstate, merged16: *const b200_frontier_entry, root_hash_mask: u16,
+                                       root_tree_mask: u16, root_kept: u16, acct_keys32: *const u8, accts: *const b200_account,
+                                       acct_flags: *const u8, m: u64, slot_keys32: *const u8, values32_be: *const u8,
+                                       seg_offsets: *const u64, mode: i32, always_include_root: i32, out: *mut b200_witness,
+                                       opt_stats: *mut b200_stats) -> i32;
     /// CPUs + preferred memory of the calling thread on the GPU's NUMA node (before allocating staging buffers)
     pub fn b200_numa_bind_thread(device_ordinal: i32) -> i32;
 }

@@ -230,6 +230,9 @@ def load():
     sig("b200_proofs_release", None, C.POINTER(Proofs))
     sig("b200_dstate_witness", i32, vp, vp, vp, vp, u64, vp, vp, vp, i32, i32, C.POINTER(Witness))
     sig("b200_witness_release", None, C.POINTER(Witness))
+    sig("b200_dstate_witness_root_kept", i32, vp, vp, vp, vp, u64, vp, vp, vp, i32, C.POINTER(C.c_uint16))
+    sig("b200_dstate_sharded_witness", i32, vp, C.POINTER(FrontierEntry), C.c_uint16, C.c_uint16, C.c_uint16, vp, vp, vp, u64, vp, vp, vp,
+        i32, i32, C.POINTER(Witness), C.POINTER(Stats))
     sig("b200_witness_roots", i32, vp, u64, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, PS)
     sig("b200_dstate_overlay_roots", i32, vp, u64, vp, vp, vp, vp, vp, vp, vp, vp, PS)
     sig("b200_dstate_overlay_frontiers", i32, vp, u64, vp, vp, vp, vp, vp, vp, vp, C.POINTER(FrontierEntry), PS)

@@ -58,6 +58,11 @@ cudaError_t launch_iota(uint32_t *out, uint64_t n, uint32_t first, cudaStream_t 
     iota_kernel<<<blocks_for(n, 256), 256, 0, st>>>(out, n, first);
     return cudaGetLastError();
 }
+cudaError_t launch_fill_u32(uint32_t *out, uint64_t n, uint32_t value, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    fill_u32_kernel<<<blocks_for(n, 256), 256, 0, st>>>(out, n, value);
+    return cudaGetLastError();
+}
 cudaError_t launch_gap_keys(const uint8_t *Lp, uint64_t G, uint16_t *key, uint32_t *val, uint32_t *unresolved, cudaStream_t st) {
     if (G == 0) return cudaSuccess;
     gap_keys_kernel<<<blocks_for(G, 256), 256, 0, st>>>(Lp, G, key, val, unresolved);

@@ -65,6 +65,10 @@ __global__ void iota_kernel(uint32_t *__restrict__ out, uint64_t n, uint32_t fir
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) out[i] = first + (uint32_t)i;
 }
+__global__ void fill_u32_kernel(uint32_t *__restrict__ out, uint64_t n, uint32_t value) {
+    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) out[i] = value;
+}
 
 // Sort input of the gaps, in position order: val[g-1] = g, key[g-1] = depth | head << 8 | unresolved << 9 (a boundary
 // gap: 0xFF, it sorts behind the real ones).  The sort looks at bits 0..7 only and is stable, so the flags travel with

@@ -137,10 +137,11 @@ static __device__ __forceinline__ bool wt_wiped(const uint8_t *flags, uint64_t i
 }
 
 // Accounts, first pass: the account leaf and the storage trie (entry_trie, nullable: the leaf) of every account entry, the
-// key order, the wiped storage tries.
+// key order, the wiped storage tries.  acct_trie (nullable: trie 0): the account trie of every entry, a bucket trie of a
+// sharded state.
 __global__ void wt_accounts_kernel(DTrieDev ta, DTrieDev ts, const uint8_t *__restrict__ keys, const uint8_t *__restrict__ flags,
-                                   uint64_t m, const uint32_t *__restrict__ entry_trie, uint32_t *__restrict__ leaf_of,
-                                   uint32_t *__restrict__ trie_of, uint8_t *__restrict__ trie_flags) {
+                                   uint64_t m, const uint32_t *__restrict__ entry_trie, const uint32_t *__restrict__ acct_trie,
+                                   uint32_t *__restrict__ leaf_of, uint32_t *__restrict__ trie_of, uint8_t *__restrict__ trie_flags) {
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= m) return;
     const uint8_t *key = keys + 32 * i;
@@ -148,7 +149,7 @@ __global__ void wt_accounts_kernel(DTrieDev ta, DTrieDev ts, const uint8_t *__re
         uint32_t l = dt_lcp(key - 32, key, 0, 64);
         if (l == 64 || dt_nib(key - 32, l) > dt_nib(key, l)) atomicExch(ta.err, B200_DEVERR_UNSORTED);
     }
-    DtLoc loc = dt_descend(ta, 0, key);
+    DtLoc loc = dt_descend(ta, acct_trie ? acct_trie[i] : 0u, key);
     const uint32_t leaf = loc.found ? (loc.child & ~DT_LEAF) : DT_NONE;
     const uint32_t trie = leaf == DT_NONE ? DT_NONE : entry_trie ? entry_trie[i] : leaf;
     leaf_of[i] = leaf;
@@ -181,10 +182,12 @@ __global__ void wt_slots_kernel(DTrieDev ts, WitnessMarks w, const uint64_t *__r
 }
 
 // Accounts, second pass (after the storage walks): removal or upsert (TrieWitness: removal iff the account is empty and
-// its storage root after the block is EMPTY_ROOT_HASH), the walk in the account trie, and the Legacy storage-root target.
+// its storage root after the block is EMPTY_ROOT_HASH), the walk in the account trie (acct_trie as wt_accounts_kernel), and
+// the Legacy storage-root target.
 __global__ void wt_account_walk_kernel(DTrieDev ta, DTrieDev ts, WitnessMarks w, const uint8_t *__restrict__ keys,
                                        const uint8_t *__restrict__ accts, const uint8_t *__restrict__ flags,
-                                       const uint64_t *__restrict__ seg_offsets, uint64_t m, const uint32_t *__restrict__ leaf_of,
+                                       const uint64_t *__restrict__ seg_offsets, uint64_t m, const uint32_t *__restrict__ acct_trie,
+                                       const uint32_t *__restrict__ leaf_of,
                                        const uint32_t *__restrict__ trie_of, const uint8_t *__restrict__ trie_flags, const uint8_t *__restrict__ nonzero, int canonical,
                                        uint32_t *__restrict__ root_trie, uint16_t *__restrict__ root_meta) {
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -207,8 +210,9 @@ __global__ void wt_account_walk_kernel(DTrieDev ta, DTrieDev ts, WitnessMarks w,
     else removal = wt_account_empty(accts + 72 * i) && post_empty;
     root_trie[i] = trie;
     root_meta[i] = (!canonical && !has_targets) ? WM_ROOT_ONLY : WM_SKIP;
-    const bool found = wt_walk(ta, w, 0, keys + 32 * i, removal, false);
-    if (canonical && !removal && !ignored && !found) wt_walk(ta, w, 0, keys + 32 * i, false, true);
+    const uint32_t at = acct_trie ? acct_trie[i] : 0u;
+    const bool found = wt_walk(ta, w, at, keys + 32 * i, removal, false);
+    if (canonical && !removal && !ignored && !found) wt_walk(ta, w, at, keys + 32 * i, false, true);
 }
 
 // Reveal targets: every listed branch with exactly one surviving child that no target walks through and whose node is
@@ -399,6 +403,61 @@ __global__ void wt_proof_write_kernel(DTrieDev t, DTrieDev res, const uint32_t *
     wt_target<true>(t, res, res_trie, trie_of, keys, meta, i, nn, nb, rlp, byte_shift + byte_base[i], rlp_offset, node_shift + node_base[i]);
 }
 
+// The account targets of a sharded state (b200_dstate_sharded_witness): t holds the 16 bucket tries and the walks start at
+// the gathered root (ShardRootDev), as dt_sharded_proof_walk does.  With the root branch (two or more non-empty buckets) it
+// is kept when min_len is 0, then the walk goes on from the top of the key's bucket at parent depth 0 (nothing more when the
+// bucket is empty); with `only` bucket only's trie is the whole trie, walked from parent depth -1 (trie 0 of an empty state
+// gives 0x80).  The bucket follows from the key; trie ids are not read.
+template <bool WRITE>
+static __device__ __forceinline__ void wt_sharded_target(const DTrieDev &t, const ShardRootDev &r, const uint8_t *__restrict__ keys,
+                                                         const uint16_t *__restrict__ meta, uint64_t i, uint32_t &nn, uint64_t &nb,
+                                                         uint8_t *rlp, uint64_t byte_base, uint64_t *rlp_offset, uint64_t node_base) {
+    const uint16_t mt = meta[i];
+    const uint8_t *key = keys + 32 * i;
+    const uint32_t min_len = mt & 0xFF, stop = mt >> 8;
+    nn = 0;
+    nb = 0;
+    if (mt & WM_SKIP) return;
+    if (r.only >= 0) {
+        dt_proof_walk<WRITE, true>(t, (uint32_t)r.only, key, nn, nb, rlp, byte_base, rlp_offset, nullptr, nullptr, node_base, min_len, stop);
+        return;
+    }
+    if (min_len == 0) {
+        const uint32_t len = *reinterpret_cast<const uint32_t *>(r.branch);
+        if (WRITE) {
+            for (uint32_t b = 0; b < len; b++) rlp[byte_base + b] = r.branch[4 + b];
+            rlp_offset[node_base] = byte_base;
+        }
+        nn = 1;
+        nb = len;
+        if (stop & (WT_ROOT_ONLY | WT_FIRST_ONLY)) return;
+    }
+    const uint32_t cur = t.troot[key[0] >> 4];
+    if (cur != DT_NONE)
+        dt_proof_steps<WRITE, true>(t, cur, 0, key, nn, nb, rlp, byte_base, rlp_offset, nullptr, nullptr, node_base, min_len, stop);
+}
+__global__ void wt_sharded_proof_size_kernel(DTrieDev t, ShardRootDev r, const uint8_t *__restrict__ keys, const uint16_t *__restrict__ meta,
+                                             uint64_t n_fixed, const uint32_t *__restrict__ n_extra, uint64_t n_max,
+                                             uint32_t *__restrict__ node_count, uint64_t *__restrict__ byte_count) {
+    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_max) return;
+    uint32_t nn = 0;
+    uint64_t nb = 0;
+    if (i < n_fixed + *n_extra) wt_sharded_target<false>(t, r, keys, meta, i, nn, nb, nullptr, 0, nullptr, 0);
+    node_count[i] = nn;
+    byte_count[i] = nb;
+}
+__global__ void wt_sharded_proof_write_kernel(DTrieDev t, ShardRootDev r, const uint8_t *__restrict__ keys, const uint16_t *__restrict__ meta,
+                                              uint64_t n_fixed, const uint32_t *__restrict__ n_extra, uint64_t n_max,
+                                              const uint64_t *__restrict__ node_base, const uint64_t *__restrict__ byte_base,
+                                              uint8_t *__restrict__ rlp, uint64_t *__restrict__ rlp_offset) {
+    uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_max || i >= n_fixed + *n_extra) return;
+    uint32_t nn;
+    uint64_t nb;
+    wt_sharded_target<true>(t, r, keys, meta, i, nn, nb, rlp, byte_base[i], rlp_offset, node_base[i]);
+}
+
 // After the sort by hash: keep[i] = 1 for the first of every run of equal hashes (Canonical: not the empty node 0x80),
 // kept_bytes[i] its length.
 __global__ void wt_unique_kernel(const uint8_t *__restrict__ sorted32, const uint32_t *__restrict__ perm, const uint64_t *__restrict__ rlp_offset,
@@ -433,8 +492,9 @@ __global__ void wt_gather_kernel(const uint8_t *__restrict__ sorted32, const uin
 
 // ------------------------------------------------------------------------------------------------ launchers
 cudaError_t launch_wt_accounts(const DTrieDev &ta, const DTrieDev &ts, const uint8_t *keys, const uint8_t *flags, uint64_t m,
-                               const uint32_t *entry_trie, uint32_t *leaf_of, uint32_t *trie_of, uint8_t *trie_flags, cudaStream_t st) {
-    if (m) wt_accounts_kernel<<<blocks_for(m, 128), 128, 0, st>>>(ta, ts, keys, flags, m, entry_trie, leaf_of, trie_of, trie_flags);
+                               const uint32_t *entry_trie, const uint32_t *acct_trie, uint32_t *leaf_of, uint32_t *trie_of,
+                               uint8_t *trie_flags, cudaStream_t st) {
+    if (m) wt_accounts_kernel<<<blocks_for(m, 128), 128, 0, st>>>(ta, ts, keys, flags, m, entry_trie, acct_trie, leaf_of, trie_of, trie_flags);
     return cudaGetLastError();
 }
 cudaError_t launch_wt_slots(const DTrieDev &ts, const WitnessMarks &w, const uint64_t *seg_offsets, uint64_t m, const uint32_t *trie_of,
@@ -444,12 +504,12 @@ cudaError_t launch_wt_slots(const DTrieDev &ts, const WitnessMarks &w, const uin
     return cudaGetLastError();
 }
 cudaError_t launch_wt_account_walk(const DTrieDev &ta, const DTrieDev &ts, const WitnessMarks &w, const uint8_t *keys, const uint8_t *accts,
-                                   const uint8_t *flags, const uint64_t *seg_offsets, uint64_t m, const uint32_t *leaf_of,
-                                   const uint32_t *trie_of, const uint8_t *trie_flags, const uint8_t *nonzero, int canonical, uint32_t *root_trie,
-                                   uint16_t *root_meta, cudaStream_t st) {
+                                   const uint8_t *flags, const uint64_t *seg_offsets, uint64_t m, const uint32_t *acct_trie,
+                                   const uint32_t *leaf_of, const uint32_t *trie_of, const uint8_t *trie_flags, const uint8_t *nonzero,
+                                   int canonical, uint32_t *root_trie, uint16_t *root_meta, cudaStream_t st) {
     if (m)
-        wt_account_walk_kernel<<<blocks_for(m, 128), 128, 0, st>>>(ta, ts, w, keys, accts, flags, seg_offsets, m, leaf_of, trie_of, trie_flags, nonzero,
-                                                                   canonical, root_trie, root_meta);
+        wt_account_walk_kernel<<<blocks_for(m, 128), 128, 0, st>>>(ta, ts, w, keys, accts, flags, seg_offsets, m, acct_trie, leaf_of, trie_of,
+                                                                   trie_flags, nonzero, canonical, root_trie, root_meta);
     return cudaGetLastError();
 }
 cudaError_t launch_wt_reveal(const DTrieDev &t, const WitnessMarks &w, uint32_t max_list, int canonical, uint32_t *out_trie,
@@ -496,6 +556,19 @@ cudaError_t launch_wt_proof_write(const DTrieDev &t, const DTrieDev &res, const 
     if (n_max)
         wt_proof_write_kernel<<<blocks_for(n_max, 64), 64, 0, st>>>(t, res, res_trie, trie_of, keys, meta, n_fixed, n_extra, n_max, node_base, byte_base,
                                                                     node_shift, byte_shift, rlp, rlp_offset);
+    return cudaGetLastError();
+}
+cudaError_t launch_wt_sharded_proof_sizes(const DTrieDev &t, const ShardRootDev &r, const uint8_t *keys, const uint16_t *meta, uint64_t n_fixed,
+                                          const uint32_t *n_extra, uint64_t n_max, uint32_t *node_count, uint64_t *byte_count, cudaStream_t st) {
+    if (n_max) wt_sharded_proof_size_kernel<<<blocks_for(n_max, 64), 64, 0, st>>>(t, r, keys, meta, n_fixed, n_extra, n_max, node_count, byte_count);
+    return cudaGetLastError();
+}
+cudaError_t launch_wt_sharded_proof_write(const DTrieDev &t, const ShardRootDev &r, const uint8_t *keys, const uint16_t *meta, uint64_t n_fixed,
+                                          const uint32_t *n_extra, uint64_t n_max, const uint64_t *node_base, const uint64_t *byte_base,
+                                          uint8_t *rlp, uint64_t *rlp_offset, cudaStream_t st) {
+    if (n_max)
+        wt_sharded_proof_write_kernel<<<blocks_for(n_max, 64), 64, 0, st>>>(t, r, keys, meta, n_fixed, n_extra, n_max, node_base, byte_base, rlp,
+                                                                            rlp_offset);
     return cudaGetLastError();
 }
 cudaError_t launch_wt_unique(const uint8_t *sorted32, const uint32_t *perm, const uint64_t *rlp_offset, const uint8_t *rlp, uint64_t n,

@@ -79,6 +79,7 @@ cudaError_t launch_mark_boundaries(const uint64_t *d_seg_offsets, uint64_t n_seg
                                    cudaStream_t st);
 cudaError_t launch_lcp(const uint8_t *keys, uint64_t n, uint8_t *Lp, uint8_t *nibs, int *err, cudaStream_t st);
 cudaError_t launch_iota(uint32_t *out, uint64_t n, uint32_t first, cudaStream_t st);
+cudaError_t launch_fill_u32(uint32_t *out, uint64_t n, uint32_t value, cudaStream_t st);
 cudaError_t launch_gap_keys(const uint8_t *Lp, uint64_t G, uint16_t *key, uint32_t *val, uint32_t *unresolved, cudaStream_t st);
 cudaError_t launch_bucket_offsets(const uint16_t *key_sorted, uint64_t G, uint32_t *bucket_off, cudaStream_t st);
 cudaError_t launch_head_fix(const uint8_t *keys, uint16_t *key_sorted, const uint32_t *gap_sorted, const uint64_t *seg_offsets,
@@ -301,20 +302,23 @@ struct WitnessMarks {       // per-call scratch of one arena
     uint32_t *seen;         // [ncap] bit c: a target walks through child c; bit 16 + c: an inserted key does (Canonical)
     uint32_t *list;         // branches that lost a child, [0, *n_list)
     uint32_t *n_list;
-    uint8_t *trie_flags;    // storage forest only, [account leaf capacity]: WF_*
+    uint8_t *trie_flags;    // WF_* per trie: storage forest [account leaf capacity]; account arena of a shard
+                            // (b200_dstate_sharded_witness) [16], WF_EMPTIED per bucket; null otherwise
 };
 // b200_dstate_overlay_witness runs these on an overlay's folds: entry_trie (nullable: the account leaf) is the storage trie of
 // every entry; res / res_trie: the resident arena, and its trie behind each trie of the fold, below the fold's hash leaves
 // (res_trie nullptr: trie 0).  On the resident arenas res is the arena itself and holds no hash leaf.
+// acct_trie (nullable: trie 0): the account trie of every entry (b200_dstate_sharded_witness: a bucket trie of the shard).
 cudaError_t launch_wt_accounts(const DTrieDev &ta, const DTrieDev &ts, const uint8_t *keys, const uint8_t *flags, uint64_t m,
-                               const uint32_t *entry_trie, uint32_t *leaf_of, uint32_t *trie_of, uint8_t *trie_flags, cudaStream_t st);
+                               const uint32_t *entry_trie, const uint32_t *acct_trie, uint32_t *leaf_of, uint32_t *trie_of,
+                               uint8_t *trie_flags, cudaStream_t st);
 cudaError_t launch_wt_slots(const DTrieDev &ts, const WitnessMarks &w, const uint64_t *seg_offsets, uint64_t m, const uint32_t *trie_of,
                             const uint8_t *flags, const uint8_t *keys, const uint8_t *vals, uint64_t n, int canonical,
                             uint32_t *trie_of_target, uint8_t *nonzero, cudaStream_t st);
 cudaError_t launch_wt_account_walk(const DTrieDev &ta, const DTrieDev &ts, const WitnessMarks &w, const uint8_t *keys, const uint8_t *accts,
-                                   const uint8_t *flags, const uint64_t *seg_offsets, uint64_t m, const uint32_t *leaf_of,
-                                   const uint32_t *trie_of, const uint8_t *trie_flags, const uint8_t *nonzero, int canonical,
-                                   uint32_t *root_trie, uint16_t *root_meta, cudaStream_t st);
+                                   const uint8_t *flags, const uint64_t *seg_offsets, uint64_t m, const uint32_t *acct_trie,
+                                   const uint32_t *leaf_of, const uint32_t *trie_of, const uint8_t *trie_flags, const uint8_t *nonzero,
+                                   int canonical, uint32_t *root_trie, uint16_t *root_meta, cudaStream_t st);
 cudaError_t launch_wt_reveal(const DTrieDev &t, const WitnessMarks &w, uint32_t max_list, int canonical, uint32_t *out_trie,
                              uint8_t *out_keys, uint16_t *out_meta, uint32_t *n_out, cudaStream_t st);
 // the wipe queue holds (node, trie) pairs: node | DT_ALT = a node of res; trie_flags nullable: every trie of trie_of is wiped
@@ -334,6 +338,12 @@ cudaError_t launch_wt_proof_write(const DTrieDev &t, const DTrieDev &res, const 
                                   const uint8_t *keys, const uint16_t *meta, uint64_t n_fixed, const uint32_t *n_extra, uint64_t n_max,
                                   const uint64_t *node_base, const uint64_t *byte_base, uint64_t node_shift, uint64_t byte_shift,
                                   uint8_t *rlp, uint64_t *rlp_offset, cudaStream_t st);
+// Account targets of a sharded state: the proofs start at the gathered root (trie ids unused, the bucket is the key's)
+cudaError_t launch_wt_sharded_proof_sizes(const DTrieDev &t, const ShardRootDev &r, const uint8_t *keys, const uint16_t *meta, uint64_t n_fixed,
+                                          const uint32_t *n_extra, uint64_t n_max, uint32_t *node_count, uint64_t *byte_count, cudaStream_t st);
+cudaError_t launch_wt_sharded_proof_write(const DTrieDev &t, const ShardRootDev &r, const uint8_t *keys, const uint16_t *meta, uint64_t n_fixed,
+                                          const uint32_t *n_extra, uint64_t n_max, const uint64_t *node_base, const uint64_t *byte_base,
+                                          uint8_t *rlp, uint64_t *rlp_offset, cudaStream_t st);
 cudaError_t launch_wt_unique(const uint8_t *sorted32, const uint32_t *perm, const uint64_t *rlp_offset, const uint8_t *rlp, uint64_t n,
                              int drop_empty, uint32_t *keep, uint64_t *kept_bytes, cudaStream_t st);
 cudaError_t launch_wt_gather(const uint8_t *sorted32, const uint32_t *perm, const uint64_t *rlp_offset, const uint8_t *rlp, uint64_t n,

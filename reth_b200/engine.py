@@ -1042,6 +1042,33 @@ class DynamicState:
             mode_id, 1 if always_include_root_node else 0, C.byref(w)))
         return self._witness_map(w)
 
+    def witness_root_kept(self, block, mode: str = "legacy") -> int:
+        """b200_dstate_witness_root_kept, on a sharded state: the 16-bit kept mask of this shard's part of a block (an `apply`
+        array tuple, entries routed by their own top nibble): bit k = bucket k still holds a leaf after the mode's removal
+        phase.  The ranks OR their masks for sharded_witness."""
+        mode_id = _witness_mode(mode)
+        k, a, f, sk, sv, so = _block_args(*block)
+        kept = C.c_uint16()
+        self.engine._check(self.engine.lib.b200_dstate_witness_root_kept(self.handle, _ptr(k), _ptr(a), _ptr(f), len(k), _ptr(sk), _ptr(sv),
+                                                                         _ptr(so), mode_id, C.byref(kept)))
+        return kept.value
+
+    def sharded_witness(self, merged, hash_mask: int, tree_mask: int, kept: int, block, mode: str = "legacy",
+                        always_include_root_node: bool = False) -> dict:
+        """b200_dstate_sharded_witness: this shard's part of the witness of a block of the whole state.  merged, hash_mask,
+        tree_mask: as for sharded_multiproof; kept: the OR of every rank's witness_root_kept; block: this rank's part (an
+        `apply` array tuple; every entry must be one this shard answers, include/b200trie.h).  always_include_root_node: only
+        when the whole block is empty.  -> {keccak(node): node RLP}; the union over the ranks is witness() of the whole block
+        on an unsharded state of all accounts."""
+        mode_id = _witness_mode(mode)
+        fr = (FrontierEntry * 16).from_buffer_copy(_np(merged).reshape(16, 68).tobytes())
+        k, a, f, sk, sv, so = _block_args(*block)
+        w, s = Witness(), Stats()
+        self.engine._check(self.engine.lib.b200_dstate_sharded_witness(
+            self.handle, fr, hash_mask, tree_mask, kept, _ptr(k), _ptr(a), _ptr(f), len(k), _ptr(sk), _ptr(sv), _ptr(so), mode_id,
+            1 if always_include_root_node else 0, C.byref(w), C.byref(s)))
+        return self._witness_map(w)
+
     def overlay_witness(self, overlay_block, block, mode: str = "legacy", always_include_root_node: bool = False) -> tuple:
         """b200_dstate_overlay_witness: the witness of `block` on the state after `overlay_block`, against the state as it is
         (the state does not change; StateProofProvider::witness of a MemoryOverlayStateProvider).  Both are `apply` array

@@ -8,7 +8,7 @@ between ranks: this is the collective-free partitioning of the reference's Paral
 (crates/trie/parallel/src/root.rs:101-127) carried over to the live path."""
 from __future__ import annotations
 
-from typing import List, Tuple
+from typing import Dict, List, Tuple
 
 import numpy as np
 
@@ -96,6 +96,32 @@ class ShardedDynamicStateRoot:
         """overlay_roots for one post: the state root `commit(post)` would return, without changing any shard."""
         return self.overlay_roots([post])[0]
 
+    def _gather_root_branch(self, extra: np.ndarray):
+        """One all-gather of every rank's 16 x 68 frontier bytes, its 4 root-mask bytes and `extra` (uint8) -> (merged (16, 68):
+        the owner's entry of every bucket, hash mask, tree mask, (world, len(extra)) every rank's extra bytes)."""
+        ds = self.local.ds
+        try:
+            hm, tm = ds.frontier_masks()
+            mine = np.concatenate([ds.frontier().reshape(-1), np.array([hm, tm], "<u2").view(np.uint8), extra])
+        except Exception as e:  # noqa: BLE001
+            raise StateRootError(str(e)) from e
+        allf = self._all_gather(mine)                                  # (world, 16 x 68 + 4 + len(extra))
+        masks = allf[:, 16 * 68:16 * 68 + 4].copy().view("<u2")        # (world, 2)
+        hash_mask, tree_mask = (int(np.bitwise_or.reduce(masks[:, i])) for i in range(2))
+        frs = allf[:, :16 * 68].reshape(self.world, 16, 68)
+        merged = np.ascontiguousarray(frs[np.arange(16) * self.world // 16, np.arange(16)])   # owner's entry of every bucket
+        return merged, hash_mask, tree_mask, allf[:, 16 * 68 + 4:]
+
+    def _answering_rank(self, merged: np.ndarray):
+        """key -> the rank that answers it: the owner of its top nibble, or in the one-bucket case of that bucket"""
+        nonempty = [k for k in range(16) if merged[k, 34]]             # as_root_len
+        def owner(key: bytes) -> int:
+            k = key[0] >> 4
+            if k not in nonempty and len(nonempty) == 1:
+                k = nonempty[0]
+            return k * self.world // 16
+        return owner
+
     def multiproof(self, targets: dict) -> dict:
         """Proof::multiproof(MultiProofTargets) of the whole state: eth_getProof and the proof workers of the state-root task
         over a sharded state.  targets: {hashed address: iterable of hashed slots}.  -> on every rank, the dict
@@ -105,22 +131,8 @@ class ShardedDynamicStateRoot:
         (b200_dstate_sharded_multiproof), and one all_gather_object of the partial dicts is merged.  At world > 1 a
         torch.distributed process group must be initialised, also when the object was made with `comm`."""
         ds = self.local.ds
-        try:
-            hm, tm = ds.frontier_masks()
-            mine = np.concatenate([ds.frontier().reshape(-1), np.array([hm, tm], "<u2").view(np.uint8)])
-        except Exception as e:  # noqa: BLE001
-            raise StateRootError(str(e)) from e
-        allf = self._all_gather(mine)                                  # (world, 16 x 68 + 4)
-        masks = allf[:, 16 * 68:].copy().view("<u2")                   # (world, 2)
-        hash_mask, tree_mask = (int(np.bitwise_or.reduce(masks[:, i])) for i in range(2))
-        frs = allf[:, :16 * 68].reshape(self.world, 16, 68)
-        merged = np.ascontiguousarray(frs[np.arange(16) * self.world // 16, np.arange(16)])   # owner's entry of every bucket
-        nonempty = [k for k in range(16) if merged[k, 34]]             # as_root_len
-        def owner(key: bytes) -> int:
-            k = key[0] >> 4
-            if k not in nonempty and len(nonempty) == 1:
-                k = nonempty[0]
-            return k * self.world // 16
+        merged, hash_mask, tree_mask, _ = self._gather_root_branch(np.zeros(0, np.uint8))
+        owner = self._answering_rank(merged)
         share = {a: s for a, s in targets.items() if owner(bytes(a)) == self.rank}
         try:
             part = ds.sharded_multiproof(merged, hash_mask, tree_mask, share)
@@ -137,6 +149,60 @@ class ShardedDynamicStateRoot:
         for p in parts:
             for name in out:
                 out[name].update(p[name])
+        return out
+
+    def witness(self, post: HashedPostState, mode: str = "legacy", always_include_root_node: bool = False) -> Dict[bytes, bytes]:
+        """TrieWitness::compute(post) of the whole state (debug_executionWitness, the invalid-block witness hook, stateless
+        clients) over a sharded state.  -> on every rank, the dict DynamicStateRoot.witness gives on one GPU; no shard
+        changes.  Raises StateRootError for a storage entry without an account entry.  Collective: every rank calls it with
+        the same post.  Each rank computes the kept mask of the block's entries in its own buckets
+        (b200_dstate_witness_root_kept); one all-gather carries it with the 16 x 68 frontier bytes, the 4 root-mask bytes and
+        a status byte; each entry then goes to the rank that answers it (as in `multiproof`; with two or more non-empty
+        buckets an entry of an empty bucket goes to every rank), each rank computes its part of the witness
+        (b200_dstate_sharded_witness), and one all_gather_object of the partial dicts, or of a rank's error, is merged.  A
+        call that fails on one rank after the frontier is read raises StateRootError on every rank, so no rank is left
+        waiting in an exchange.  At world > 1 a torch.distributed process group must be initialised, also when the object
+        was made with `comm`."""
+        from .engine import _witness_mode
+        _witness_mode(mode)                                            # a bad mode: ValueError on every rank alike
+        for k in post.storages:
+            if k not in post.accounts:
+                raise StateRootError(f"missing account {k.hex()}")
+        ds = self.local.ds
+        part = lambda keep: HashedPostState({k: a for k, a in post.accounts.items() if keep(k)},
+                                            {k: s for k, s in post.storages.items() if keep(k)})
+        kept, error = 0, None
+        try:
+            kept = ds.witness_root_kept(apply_layout(self._part(post), destroyed_slots=True)[1], mode)
+        except Exception as e:  # noqa: BLE001
+            error = str(e)
+        extra = np.concatenate([np.array([kept], "<u2").view(np.uint8), np.array([error is not None], np.uint8)])
+        merged, hash_mask, tree_mask, extras = self._gather_root_branch(extra)
+        failed = [r for r in range(self.world) if extras[r, 2]]
+        if failed:
+            raise StateRootError(error if error is not None else f"witness: the kept pre-pass failed on rank {failed[0]}")
+        root_kept = int(np.bitwise_or.reduce(extras[:, :2].copy().view("<u2")[:, 0]))
+        owner = self._answering_rank(merged)
+        every_rank = sum(1 for k in range(16) if merged[k, 34]) >= 2      # an entry of an empty bucket goes to every rank
+        mine = lambda k: owner(k) == self.rank or (every_rank and not merged[k[0] >> 4, 34])
+        block = apply_layout(part(mine), destroyed_slots=True)[1]
+        whole_block_empty = not post.accounts and not post.storages
+        try:
+            result = ds.sharded_witness(merged, hash_mask, tree_mask, root_kept, block, mode,
+                                        always_include_root_node=always_include_root_node and whole_block_empty)
+        except Exception as e:  # noqa: BLE001
+            result = f"rank {self.rank}: {e}"
+        parts = [result]
+        if self.world > 1:
+            import torch.distributed as dist
+            parts = [None] * self.world
+            dist.all_gather_object(parts, result, group=self.group)
+        errors = [p for p in parts if isinstance(p, str)]
+        if errors:
+            raise StateRootError(errors[0])
+        out = {}
+        for p in parts:
+            out.update(p)
         return out
 
     def close(self):

@@ -11,7 +11,16 @@ and the Python mirror that also builds the result dict.  For comparison it times
 account and slot keys (without the wipe expansion and the reveals).  It reports the node count, the witness bytes and the kernel
 launches of one call; --cpu-sample N also times the test-side model of tests/test_gpu_witness.py on an N-account state
 with a block scaled down in proportion (the model holds the whole state as Python tries, so it cannot take the full size).
-Prints one JSON line."""
+Prints one JSON line.
+
+    python tools/witness_bench.py --accounts 1000000 --slots 16 --touch 2000 --shards 4
+
+--shards N seeds the same state once unsharded and once as N shards on the same GPU (rank r owns the top nibbles
+[16r/N, 16(r+1)/N)) and times, alternating rep by rep, b200_dstate_witness of the block on the unsharded state and every
+shard's b200_dstate_witness_root_kept (its kept pre-pass) plus b200_dstate_sharded_witness of its part (Legacy mode): CUDA-
+event time per shard, the slowest shard and the sum over the shards (they run one after another here; on one GPU per rank
+side by side), and the launches of each call.  The merged map is checked against the unsharded one in both modes.  Reads the
+card's name, power limit and SM clock in the same run.  Prints one JSON line."""
 import argparse
 import json
 import os
@@ -107,7 +116,10 @@ def main():
     ap.add_argument("--reps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--cpu-sample", type=int, default=0, help="accounts of the state the CPU model is timed on (0 = skip)")
+    ap.add_argument("--shards", type=int, default=0, help="time the witness of a state sharded this many ways (0 = unsharded only)")
     args = ap.parse_args()
+    if args.shards:
+        return sharded_main(args)
     import torch
 
     from reth_b200 import DynamicState, Engine
@@ -196,6 +208,120 @@ def main():
     print(json.dumps(out))
     ds.close()
     eng.close()
+
+
+def sharded_main(args):
+    S = args.shards
+    if not 1 <= S <= 16:
+        raise SystemExit("--shards: 1 to 16")
+    import ctypes as C
+
+    import torch
+
+    from reth_b200 import DynamicState, Engine
+    from reth_b200._lib import FrontierEntry, Witness
+    from reth_b200.engine import _ptr
+    from tools.stateless_bench import card, spread
+    out = {"card": card()}
+    eng = Engine(0)
+    keys, accs, skeys, svals, offs = make_state(np.random.default_rng(3), args.accounts, args.slots)
+    ds = DynamicState.create(eng, keys, accs, skeys, svals, offs)
+    owner = lambda k: (k[:, 0].astype(np.int64) >> 4) * S // 16
+    bounds = np.searchsorted(owner(keys), np.arange(S + 1))           # keys are sorted: every shard holds a run of them
+
+    def state_part(r):
+        lo, hi = int(bounds[r]), int(bounds[r + 1])
+        so = offs[lo:hi + 1]
+        return keys[lo:hi], accs[lo:hi], skeys[int(so[0]):int(so[-1])], svals[int(so[0]):int(so[-1])], so - so[0]
+    shards = [DynamicState.create(eng, *state_part(r), sharded=True) for r in range(S)]
+    merged = np.zeros((16, 68), np.uint8)
+    hm = tm = 0
+    for r, d in enumerate(shards):
+        mine = [b for b in range(16) if b * S // 16 == r]
+        merged[mine] = d.frontier()[mine]
+        h, t = d.frontier_masks()
+        hm, tm = hm | h, tm | t
+    assert eng.root_from_frontier(merged) == ds.root()
+    block = make_block(np.random.default_rng(77), keys, skeys, offs, args.touch, args.slot_writes)
+    arrays = block_arrays(block)
+    parts = [block_arrays({k: v for k, v in block.items() if (k[0] >> 4) * S // 16 == r}) for r in range(S)]
+    out.update({"accounts": args.accounts, "slots": args.accounts * args.slots, "shards": S, "block_accounts": len(arrays[0]),
+                "block_slot_entries": len(arrays[3]), "block_accounts_per_shard": [len(p[0]) for p in parts]})
+    fr = (FrontierEntry * 16).from_buffer_copy(merged.tobytes())
+    kept_of = {}
+
+    def kept_call(r, mode=0):
+        bk, ba, bf, bsk, bsv, bso = parts[r]
+        kept = C.c_uint16()
+        eng._check(eng.lib.b200_dstate_witness_root_kept(shards[r].handle, _ptr(bk), _ptr(ba), _ptr(bf), len(bk), _ptr(bsk), _ptr(bsv),
+                                                         _ptr(bso), mode, C.byref(kept)))
+        return kept.value
+
+    def witness_call(r=None, mode=0):  # the C ABI call alone (the Python dict of the result is not built)
+        bk, ba, bf, bsk, bsv, bso = arrays if r is None else parts[r]
+        w = Witness()
+        if r is None:
+            rc = eng.lib.b200_dstate_witness(ds.handle, _ptr(bk), _ptr(ba), _ptr(bf), len(bk), _ptr(bsk), _ptr(bsv), _ptr(bso), mode, 0,
+                                             C.byref(w))
+        else:
+            rc = eng.lib.b200_dstate_sharded_witness(shards[r].handle, fr, hm, tm, kept_of[mode], _ptr(bk), _ptr(ba), _ptr(bf), len(bk),
+                                                     _ptr(bsk), _ptr(bsv), _ptr(bso), mode, 0, C.byref(w), None)
+        eng._check(rc)
+        n = int(w.n)
+        eng.lib.b200_witness_release(C.byref(w))
+        return n
+
+    for mode in (0, 1):
+        kept_of[mode] = 0
+        for r in range(S):
+            kept_of[mode] |= kept_call(r, mode)
+    calls = {"unsharded": lambda: witness_call()}
+    for r in range(S):
+        calls[f"kept_{r}"] = lambda r=r: kept_call(r)
+        calls[f"witness_{r}"] = lambda r=r: witness_call(r)
+    launches = {}
+    for k, c in calls.items():
+        l0 = eng.launch_count()
+        c()
+        launches[k] = eng.launch_count() - l0
+    stream = torch.cuda.current_stream()
+    eng.set_stream(stream.cuda_stream)
+    ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    for _ in range(args.warmup):
+        for c in calls.values():
+            c()
+    dev = {k: [] for k in calls}
+    for _ in range(args.reps):
+        for k, c in calls.items():
+            torch.cuda.synchronize()
+            ev0.record(stream)
+            c()
+            ev1.record(stream)
+            ev1.synchronize()
+            dev[k].append(ev0.elapsed_time(ev1))
+    kd, wd = np.array([dev[f"kept_{r}"] for r in range(S)]), np.array([dev[f"witness_{r}"] for r in range(S)])
+    out["unsharded_witness"] = {"device_ms": spread(dev["unsharded"]), "launches": launches["unsharded"]}
+    out["sharded_witness"] = {
+        "per_shard": [{"kept_ms": spread(dev[f"kept_{r}"]), "witness_ms": spread(dev[f"witness_{r}"]),
+                       "kept_launches": launches[f"kept_{r}"], "witness_launches": launches[f"witness_{r}"]} for r in range(S)],
+        "max_over_shards_ms": spread((kd + wd).max(axis=0)), "sum_over_shards_ms": spread((kd + wd).sum(axis=0)),
+        "kept_share_of_sum": round(float(np.median(kd.sum(axis=0)) / np.median((kd + wd).sum(axis=0))), 3)}
+    matches = {}
+    for mode in ("legacy", "canonical"):
+        kept = 0
+        for r in range(S):
+            kept |= shards[r].witness_root_kept(parts[r], mode)
+        union = {}
+        for r in range(S):
+            union.update(shards[r].sharded_witness(merged, hm, tm, kept, parts[r], mode))
+        matches[mode] = union == ds.witness(*arrays, mode=mode)
+    out["matches_unsharded"] = matches
+    for d in shards + [ds]:
+        d.close()
+    eng.close()
+    print(json.dumps(out))
+    if not all(matches.values()):
+        raise SystemExit("the merged sharded witness differs from the unsharded one")
 
 
 if __name__ == "__main__":
